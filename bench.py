@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Benchmark of the FILM hot path: interpolated frames/sec (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 \
         --master-port P bench.py --gpus N --steps K --warmup W
 
@@ -14,9 +14,14 @@ own frame pairs (frame pairs shard embarrassingly; no data-path collective) -> w
 `e2e`     : frames/s through the reference-facing API `Interpolator.__call__(x0, x1, dt)` with
             pinned HOST numpy buffers; H2D of both frames and D2H of the result are inside
             the timed region.
-`roofline`: conv implicit-GEMM kernels (tcgen05), reference-graph FLOPs / summed kernel time
+`roofline`: conv implicit-GEMM kernels (wgmma), reference-graph FLOPs / summed kernel time
             measured with one CUDA-event pair per launch in a separate eager pass, against
-            the measured bf16 peak of MEASURED_PEAKS.json.
+            the bf16 peak of MEASURED_PEAKS.json or, without it, the H100 SXM data-sheet figure.
+`--dump-outputs DIR`: after the timed steps, the interpolated frame of the last timed step (what a caller of
+            film_interpolate_device receives) is written as DIR/interpolated_frame.npy (float32, 1x1080x1920x3 at
+            the default size); a frame over 64 MB is written as a fixed seeded sample of its pixels instead
+            (interpolated_frame_sample.npy + _pixels.npy). The inputs are seeded, so two builds can be compared
+            output for output.
 `workloads`: the other BASELINE.json configs, in the same JSON line: 4K tiled 2x2 (configs[2]),
             8K tiled 4x4 with the tiles sharded over the ranks and ONE NCCL all-gather inside the
             timed region (configs[4]), 720p recursive x6 = 63 mid-frames scheduled level-synchronously
@@ -55,8 +60,8 @@ def load_peaks():
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0,
+            "source": "H100 SXM data sheet (dense bf16, HBM3), not measured"}
 
 
 class ClockSampler:
@@ -127,9 +132,6 @@ class ClockSampler:
 
 _BEST_THREADS = None
 REF_WALL_BUDGET_S = 200.0      # the reference arm must end "within a few minutes"
-# DRAM bytes (read + write) of the tensor-core conv launches of ONE 1080p call, summed from the committed ncu capture
-# profiles/r2l_ncu_counters_1080p.csv (tools/gpu_final_r2.sh: `ncu --metrics dram__bytes_read.sum,dram__bytes_write.sum,...`)
-NCU_CONV_DRAM_BYTES_PER_STEP = 20.209e9
 
 
 def _pick_threads():
@@ -346,6 +348,24 @@ class _solo:
         self.p._world_rank = self.saved
 
 
+DUMP_BUDGET_BYTES = 64 << 20
+
+
+def dump_frame(out_dir, frame):
+    """The interpolated frame as float32 .npy: whole while it fits DUMP_BUDGET_BYTES, otherwise a fixed sample of pixels
+    (seeded, sorted flat pixel indices, all three channels) with the indices beside it."""
+    os.makedirs(out_dir, exist_ok=True)
+    frame = np.ascontiguousarray(frame, dtype=np.float32)
+    if frame.nbytes <= DUMP_BUDGET_BYTES:
+        np.save(os.path.join(out_dir, "interpolated_frame.npy"), frame)
+        return
+    pix = frame.reshape(-1, frame.shape[-1])
+    n = DUMP_BUDGET_BYTES // 2 // (pix.shape[1] * 4)    # half the budget for the values, the rest covers the indices
+    idx = np.sort(np.random.default_rng(0).choice(pix.shape[0], size=n, replace=False))
+    np.save(os.path.join(out_dir, "interpolated_frame_sample.npy"), pix[idx])
+    np.save(os.path.join(out_dir, "interpolated_frame_sample_pixels.npy"), idx.astype(np.float64))   # exact below 2^53
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -357,6 +377,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-workloads", action="store_true", help="skip the 4K / 8K / 720p-recursive workloads")
     ap.add_argument("--op-table", default=None, help="write the per-kernel timing table (csv) here")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's interpolated frame as DIR/interpolated_frame.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -412,6 +434,8 @@ def main():
         e1.record(stream)
         barrier()
         ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_frame(args.dump_outputs, dout.cpu().numpy())
     t_ms = torch.tensor([ms], device=dev, dtype=torch.float64)
     if world > 1:
         dist.all_reduce(t_ms, op=dist.ReduceOp.MAX)
@@ -490,16 +514,14 @@ def main():
     three_pass = [n for i, n in enumerate(names) if not (mask >> i) & 1]
     ach_tf = conv_flops / (conv_ms * 1e-3) / 1e12
     roofline = {
-        "bound": "tensor", "kernel": "k_conv_tc<BN> (tcgen05 implicit-GEMM conv, all call sites)",
+        "bound": "tensor", "kernel": "k_conv_tc / k_conv3x3_tc (wgmma implicit-GEMM conv, all call sites)",
         "achieved": ach_tf, "peak": peaks["bf16_tflops_sustained"], "unit": "TFLOP/s",
-        "frac": ach_tf / peaks["bf16_tflops_sustained"], "traffic": NCU_CONV_DRAM_BYTES_PER_STEP,
-        "traffic_note": "dram__bytes_read.sum + dram__bytes_write.sum summed over the 76 tensor-core conv launches of one 1080p "
-                        "call, ncu capture of build r2l (profiles/r2l_ncu_counters_1080p.csv; dominant launch fusion_conv1@L1: "
-                        "1.55 GB in 1.24 ms, tensor pipe 79 %; conv launches = 82.8 % of the step under ncu, 82.0 % by CUDA events); `algorithmic_bytes_per_step` is the engine's own count (every "
-                        "source plane a call site consumes read once, every destination plane written once)",
+        "frac": ach_tf / peaks["bf16_tflops_sustained"],
+        "traffic_note": "`algorithmic_bytes_per_step` is the engine's own count (every source plane a call site consumes "
+                        "read once, every destination plane written once)",
         "algorithmic_bytes_per_step": sum(a["alg_bytes"] for a in conv),
-        "peak_source": peaks["source"] + ", sustained bf16 cuBLAS",
-        "mma_kind": "tcgen05.mma kind::f16 (fp16 operands, fp32 accumulate); per-stage precision plan: 1 pass (hi*hi) on "
+        "peak_source": peaks["source"],
+        "mma_kind": "wgmma.mma_async f32.f16.f16 (fp16 operands, fp32 accumulate); per-stage precision plan: 1 pass (hi*hi) on "
                     + ",".join(one_pass) + "; 3 passes (hi*hi + hi*lo + lo*hi) on " + ",".join(three_pass) + " and the heads",
         "onepass_mask": hex(mask),
         "issued_tflops": prof["mma_flops"] / (conv_ms * 1e-3) / 1e12,
@@ -534,7 +556,7 @@ def main():
                                f"{w}x{h} single mid-frame, Style architecture, batch 1, align 64 -> {prof['padded_h']}x{prof['padded_w']}",
                    "per_gpu": "one frame pair per GPU per step",
                    "weights": "synthetic seed 1234 (random-init Style architecture)",
-                   "l2": f"per-step working set {prof['arena_bytes'] / 1e9:.1f} GB >> 126 MB L2 (no flush needed)",
+                   "l2": f"per-step working set {prof['arena_bytes'] / 1e9:.1f} GB >> 50 MB L2 (no flush needed)",
                    "parallelism": f"frame-pair sharding x{world} (one process per GPU, no data-path collective)",
                    "cuda_graph": bool(prof["used_graph"])},
         "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": 2 * frame_bytes,

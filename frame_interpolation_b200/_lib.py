@@ -41,7 +41,7 @@ def load() -> C.CDLL:
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"{LIB_PATH} not found: build it with `python -m frame_interpolation_b200.build` "
-            "(the FILM B200 engine has no CPU fallback)")
+            "(the FILM engine has no CPU fallback)")
     lib = C.CDLL(LIB_PATH)
     fp = C.POINTER(C.c_float)
     lib.film_create.argtypes = [C.POINTER(C.c_void_p), C.c_char_p, C.c_int]

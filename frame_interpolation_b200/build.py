@@ -1,4 +1,4 @@
-"""Builds libfilm_b200.so in-tree with nvcc for sm_100a (no torch, no cmake).
+"""Builds libfilm_b200.so in-tree with nvcc for sm_90a (no torch, no cmake).
 
     python -m frame_interpolation_b200.build [--force] [--verbose]
 
@@ -17,13 +17,13 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-SOURCES = ["film_engine.cu", "film_kernels.cu", "film_conv_tc.cu", "film_conv3x3_tc.cu", "film_conv3x3_tc2.cu"]
+SOURCES = ["film_engine.cu", "film_kernels.cu", "film_conv_tc.cu", "film_conv3x3_tc.cu"]
 HEADERS = ["film_common.cuh", "film_conv.h", "film_kernels.h", "film_tc_ptx.cuh", os.path.join("..", "..", "include", "film_b200.h")]
 LIB = os.path.join(HERE, "libfilm_b200.so")
 STAMP = os.path.join(HERE, "_build", "stamp")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
     "--expt-relaxed-constexpr",

@@ -1,10 +1,10 @@
-// Shared device/host definitions of the FILM B200 engine.
+// Shared device/host definitions of the FILM engine.
 //
 // Activation storage ("split" format): every feature tensor is NHWC and stored as TWO
 // 16-bit planes, hi = rn16(x) and lo = rn16(x - hi).  Same bytes as fp32, but each plane
-// is directly consumable by tcgen05.mma kind::f16, and hi + lo carries 16 mantissa bits
+// is directly consumable by wgmma (f16 / bf16 operands), and hi + lo carries 16 mantissa bits
 // (bf16) -- the 3-pass product  A_hi*W_hi + A_hi*W_lo + A_lo*W_hi  then matches an fp32
-// convolution to ~1e-5 relative (measured against the fp64 oracle, DESIGN.md section 3).
+// convolution to ~1e-5 relative (measured against the fp64 oracle).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -53,7 +53,7 @@ __device__ __forceinline__ void split2(float x, sp_t& hi, sp_t& lo) {
 // two floats -> packed hi pair / lo pair (little-endian: element 0 in the low half)
 #ifndef FILM_SPLIT_FP16
 // bf16: one packed convert per plane (F2FP.BF16.F32.PACK_AB), float(bf16) is a 16-bit shift -> 6
-// instructions per pair (the gather kernels are instruction-issue bound, ncu profiles/r1o)
+// instructions per pair (the gather kernels are instruction-issue bound)
 __device__ __forceinline__ void split_pack2(float a, float b, uint32_t& hi, uint32_t& lo) {
   const __nv_bfloat162 h2 = __floats2bfloat162_rn(a, b);
   hi = *reinterpret_cast<const uint32_t*>(&h2);
@@ -116,18 +116,17 @@ __device__ __forceinline__ void pack8(const float* v, uint4& h, uint4& l) {
   split_pack2(v[6], v[7], h.w, l.w);
 }
 
-// 256-bit global accesses (sm_100: LDG/STG.E.ENL2.256): 16 channels of one plane per instruction, i.e.
-// one whole 32-byte sector per thread -- the strided per-pixel epilogue stores and the gathers are
-// instruction-issue / LSU bound, not bandwidth bound.  Addresses must be 32-byte aligned.
+// 32-byte global accesses: 16 channels of one plane as two 128-bit accesses (sm_90 has no 256-bit load/store).
+// Addresses must be 16-byte aligned.
 __device__ __forceinline__ void st256(void* p, const uint4& a, const uint4& b) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(a.x), "r"(a.y), "r"(a.z),
-               "r"(a.w), "r"(b.x), "r"(b.y), "r"(b.z), "r"(b.w)
-               : "memory");
+  uint4* q = reinterpret_cast<uint4*>(p);
+  q[0] = a;
+  q[1] = b;
 }
 __device__ __forceinline__ void ld256_nc(const void* p, uint4& a, uint4& b) {
-  asm volatile("ld.global.nc.v8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-               : "l"(p));
+  const uint4* q = reinterpret_cast<const uint4*>(p);
+  a = __ldg(q);
+  b = __ldg(q + 1);
 }
 // 16 consecutive channels: pack to (hi 32 B, lo 32 B) and store
 __device__ __forceinline__ void pack_store16(const float* v, sp_t* hi_dst, sp_t* lo_dst) {

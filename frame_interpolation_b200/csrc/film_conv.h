@@ -1,4 +1,4 @@
-// Convolution problem descriptor shared by the tcgen05 implicit-GEMM kernel
+// Convolution problem descriptor shared by the wgmma implicit-GEMM kernels
 // (film_conv_tc.cu) and the CUDA-core validation kernel (film_kernels.cu).
 //
 // A "problem" is one Conv2D call site of the reference graph
@@ -40,7 +40,7 @@ struct alignas(64) ConvProblem {
   CUtensorMap tm_a_lo[kMaxSrc];
   CUtensorMap tm_w_hi;
   CUtensorMap tm_w_lo;
-  CUtensorMap tm_w_hi_half;  // box [BN/2 x KC]: CTA-pair kernel, each CTA loads half of the weight rows
+  CUtensorMap tm_w_hi_half;  // box [BN/2 x KC]: CTA-pair kernel, each CTA loads (and multicasts) half of every tap
   CUtensorMap tm_w_lo_half;
   ConvSrc src[kMaxSrc];
   int nsrc;
@@ -93,22 +93,18 @@ struct alignas(64) ConvProblem {
   sp_t* pool_lo;
   int pool_C;
   int group;              // generic kernel: number of consecutive problems launched as grid.z
-  int pair;               // 1: run on the CTA-pair (cta_group::2) persistent kernel (film_conv3x3_tc2.cu)
-  int halo;               // persistent 3x3 kernels, 16x8 tiles, 64-channel chunks: 1 = ONE (64 ch, 10 px, 18 rows)
-                          // halo box per chunk serves all nine taps (UMMA descriptors start at pixel granularity,
-                          // SBO = 1280 B; tools/ubench/desc_offset_test.cu); 0 = three dx-shifted 8-px boxes.
-                          // Set to 1 by the engine to ALLOW it; the plan functions keep or clear it.
+  int pair;               // 1: persistent 3x3 kernel as (2,1,1) clusters sharing streamed weight taps by TMA multicast
+  int halo;               // persistent 3x3 kernel, 16x8 tiles: 1 = ONE (KC ch, 10 px, 18 rows) halo box per chunk serves
+                          // all nine taps (descriptors start at pixel granularity, SBO = 10 pixel rows); 0 = three
+                          // dx-shifted 8-px boxes.  Set to 1 by the engine to ALLOW it; the plan functions keep or clear it.
   int bn;                 // N tile (32/64/128/256): conv_tc_block_n(cout), or smaller on tiny levels so that
                           // a K-serial problem spreads over more SMs
   int passes;             // MMAs per product: 3 = A_hi*W_hi + A_hi*W_lo + A_lo*W_hi (fp32-grade), 1 = A_hi*W_hi only
                           // (11-bit fp16 operands, fp32 accumulate; only the hi planes of the activations and
                           // weights are loaded).  Chosen per call site by the engine's precision plan
-                          // (film_engine.cu, DESIGN.md section 3).
-  int straight;           // persistent kernels, resident weights: 1 = one elected lane issues a whole activation stage as
-                          // straight-line code (default), 0 = per-tap issue loop
-  int dual;               // CTA-pair kernel, streamed weights, wide halo: 1 = every weight tap pulled from L2 serves TWO
-                          // spatial work items (their activation stages are resident together, two accumulator
-                          // sets in TMEM): halves the weight bytes per item where the layer is L2->SM ingest bound
+                          // (film_engine.cu).
+  int straight;           // persistent kernel, resident weights: 1 = a whole activation stage is one wgmma group issued as
+                          // straight-line code (default), 0 = one group per tap
   int out_lo_skip;        // 1: every consumer of the destination reads the hi plane only -> the lo plane is not written
 };
 
@@ -117,13 +113,9 @@ cudaError_t launch_conv_tc(const ConvProblem* d_prob, const ConvProblem& h_prob,
 cudaError_t launch_conv_simt(const ConvProblem* d_prob, const ConvProblem& h_prob, cudaStream_t st);
 cudaError_t conv_tc_configure();  // cudaFuncSetAttribute for all instantiations
 // persistent 3x3 variant: fills the v2_* fields of `h_prob` (call before uploading the problem)
-void conv3x3_tc_plan(ConvProblem& h_prob, int num_sms);
-void conv3x3_tc_pick_tile(int H, int W, int B, int cout, int num_sms, int& tile_h, int& tile_w);
+bool conv3x3_tc_plan(ConvProblem& h_prob, int num_sms);   // false if the shape's smem rings cannot fit
+void conv3x3_tc_pick_tile(int H, int W, int B, int cout, int kc, int passes, int ktot, int epi_mode, int num_sms,
+                          int& tile_h, int& tile_w);
 cudaError_t launch_conv3x3_tc(const ConvProblem* d_prob, const ConvProblem& h_prob, cudaStream_t st);
 cudaError_t conv3x3_tc_configure();
-// CTA-pair (cta_group::2, M = 256) variant: two vertically adjacent 16x8 tiles per work item
-bool conv3x3_tc2_plan(ConvProblem& h_prob, int num_sms);  // false if the problem is not eligible
-cudaError_t launch_conv3x3_tc2(const ConvProblem* d_prob, const ConvProblem& h_prob, cudaStream_t st);
-cudaError_t conv3x3_tc2_configure();
-
 }  // namespace film

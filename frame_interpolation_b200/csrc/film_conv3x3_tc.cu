@@ -1,27 +1,23 @@
-// Persistent tcgen05 3x3 convolution with activation-tile reuse across taps (sm_100a).
+// Persistent wgmma 3x3 convolution with activation-tile reuse across taps (sm_90a).
 //
-// Why a second kernel: ncu on the generic kernel (profiles/r1_ncu_conv.md) shows the N <= 64
-// layers re-loading the same activation pixels once per tap (9 x 32 KiB per 64-channel chunk and
-// tile) and serialising prologue / mainloop / epilogue per tile.  Here:
+// Why a second kernel: the generic kernel re-loads the same activation pixels once per tap (9 x 32 KiB per
+// 64-channel chunk and tile) and serialises prologue / mainloop / epilogue per tile.  Here:
 //
 //  * Tile = 16 rows x 8 columns of output pixels.  For a 64-channel chunk the producer loads
 //    THREE boxes (dx = -1, 0, +1), each (64 ch, 8 px, 18 rows) of both planes: 144 pixel rows
 //    of 128 B = 18 KiB per plane.  Because a tile row is exactly one 1024-byte swizzle atom
 //    (8 px x 128 B), the operand of tap (dy, dx) is the SAME smem box at byte offset dy * 1024:
-//    3 loads serve 9 taps (2.67x less L2 -> smem traffic) with plain, 1024-aligned UMMA descriptors.
-//  * Weights: if the whole [Cout x K] hi+lo matrix fits (<= 144 KiB: 64->64, 128->32, 64->32 ...)
-//    it is loaded ONCE per CTA and stays resident; otherwise it streams through its own ring,
-//    one tap ([BN x 64] hi+lo) per stage.
-//  * Persistent CTAs (grid = #SMs) walk a static tile list; the fp32 accumulator is double-buffered
-//    in TMEM so the epilogue of tile i overlaps the MMAs of tile i+1.
-//  * Fused-N product (BN <= 128): every M=128,K=16 SS-mode tcgen05.mma costs >= 72 cycles whatever
-//    N <= 128 is (tools/ubench/mma_bench.cu, measured), so the 3-pass product is issued as TWO
-//    instructions per k-step:  A_hi x [W_hi ; W_lo]  (N = 2*BN, the two weight planes are contiguous
-//    in smem) and  A_lo x W_hi  accumulating into columns [0,BN).  The epilogue adds the halves.
+//    3 loads serve 9 taps (2.67x less L2 -> smem traffic) with plain, 1024-aligned descriptors.
+//  * Weights: if the whole [Cout x K] hi+lo matrix fits (64->64, 128->32, 64->32 ...) it is loaded ONCE per CTA
+//    and stays resident; otherwise it streams through its own ring, one tap ([BN x 64] hi+lo) per stage.
+//  * Persistent CTAs (grid = #SMs) walk a static tile list; the producer runs ahead into the next tile's stages while
+//    the consumers drain the accumulators of the current one.
+//  * Two-accumulator product (BN <= 128): A_hi x W_hi and A_lo x W_hi accumulate into columns [0, BN) and A_hi x W_lo
+//    into columns [BN, 2 BN) of one register accumulator, all as N = BN wgmma; the epilogue adds the halves.
 //
-// Roles (all role loops are warp-uniform, one elected lane issues): warp 0 = TMA producer
-// (+ L2 prefetch of the next tile's boxes), warp 1 = TMEM allocator + MMA issuer, warps 2-9 = epilogue
-// (two warps per TMEM lane quarter, alternating 16-column chunks).
+// Roles: warp 8 (warpgroup 2, registers handed to the consumers) = TMA producer (+ L2 prefetch of the next tile's boxes; warp-uniform, one elected lane issues),
+// warps 0-7 = two consumer warpgroups, each owning 64 pixels of the tile: wgmma into register accumulators, then the
+// epilogue straight from the registers.
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -35,20 +31,18 @@ namespace film {
 namespace {
 using namespace tc;
 
-constexpr int kEpiWarps = 8;
-constexpr int kThreads = 64 + 32 * kEpiWarps;
+constexpr int kConsumers = 256;
+constexpr int kThreads = kConsumers + 128;   // + the producer warpgroup (one active warp)
 // Tile shapes: tile_w must be a multiple of 8 pixels (one swizzle atom) and tile_h * tile_w = 128.
 // 16x8 has the smallest halo (18/16); 8x16 and 4x32 exist to avoid wave quantisation on small levels.
 __host__ __device__ constexpr int a_plane_bytes(int kc, int th, int tw) { return (th + 2) * tw * kc * 2; }
 __host__ __device__ constexpr int a_stage_bytes(int kc, int th, int tw) { return 2 * a_plane_bytes(kc, th, tw); }
-// Wide-halo mode (16x8 tiles, 64-channel chunks): ONE box (64 ch, 10 px, 18 rows) per plane and chunk serves
-// all nine taps -- the UMMA descriptor of tap (dy, dx) starts (dy * 10 + dx) * 128 B into the box and steps
-// 1280 B between 8-row groups (hardware check: tools/ubench/desc_offset_test.cu).  2.4x less L2 -> smem
-// activation traffic than the three dx-shifted boxes.
+// Wide-halo mode (16x8 tiles): ONE box (KC ch, 10 px, 18 rows) per plane and chunk serves all nine taps -- the
+// descriptor of tap (dy, dx) starts (dy * 10 + dx) pixel rows into the box and steps 10 pixel rows between 8-row
+// groups.  2.4x less L2 -> smem activation traffic than the three dx-shifted boxes.
 constexpr int kHaloW = 10, kHaloRows = 18;
 __host__ __device__ constexpr int halo_box_bytes(int kc) { return kHaloRows * kHaloW * kc * 2; }  // 23,040 for KC = 64
 __host__ __device__ constexpr int halo_plane_bytes(int kc) { return (halo_box_bytes(kc) + 1023) & ~1023; }  // 1 KiB-aligned planes
-__host__ __device__ constexpr int halo_stage_bytes(int kc) { return 2 * halo_plane_bytes(kc); }
 // `planes` = 2 (hi + lo, three-pass product) or 1 (single-pass layers load the hi planes only)
 __host__ __device__ constexpr int a_stage_bytes_h(int kc, int th, int tw, int halo, int planes = 2) {
   return planes * (halo ? halo_plane_bytes(kc) : a_plane_bytes(kc, th, tw));
@@ -57,29 +51,31 @@ constexpr int kMaxRing = 8;
 constexpr int kSmemLimit = 227 * 1024;
 constexpr int kBarBytes = 8 * (4 * kMaxRing + 4);
 constexpr int kFixedBytes = kBarBytes + 16 + 512 * 4 /*bias*/ + 64 /*src table: 16 ints*/ + 1024 /*align*/ + 64;
-// flow-head epilogue (epi_mode 3): partial sums [32 hidden][128 rows] + W3 [64][32] + b3 / W4 / b4, after the src table
-constexpr int kHeadPart = 32 * 128 * 4, kHeadW3 = 64 * 32 * 4, kHeadMisc = 512;
-constexpr int kHeadBytes = kHeadPart + kHeadW3 + kHeadMisc;
+// flow-head epilogue (epi_mode 3): W3 [64][32] + b3 / W4 / b4, after the src table
+constexpr int kHeadW3 = 64 * 32 * 4, kHeadMisc = 512;
+constexpr int kHeadBytes = kHeadW3 + kHeadMisc;
 
 __host__ __device__ inline int w_tap_bytes(int bn, int kc, int planes = 2) { return bn * kc * 2 * planes; }  // [BN x KC] hi (+ lo)
 
-template <int BN, int KC>
+// Variants are template parameters chosen on the host (launch_conv3x3_tc): kPartial = some source's trailing 16-channel
+// k-steps are zero padding in every chunk (ConvSrc::ksteps < KC/16: the 10-of-64 "side" source, the 3-of-32 image
+// block) and are skipped; kHalo = wide halo boxes; kOne = single-pass product A_hi x W_hi (hi planes only);
+// kRes = resident weights issued as straight-line code (a whole activation stage is one wgmma group).
+template <int BN, int KC, bool kPartial, bool kHalo, bool kOne, bool kRes>
 __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* __restrict__ prob) {
   extern __shared__ uint8_t smem_raw[];
-  const bool one = prob->passes == 1;   // single-pass product A_hi x W_hi: hi planes only
+  constexpr bool one = kOne;
   const int planes = one ? 1 : 2;
   constexpr int kWPlane = BN * KC * 2;  // one weight plane of one tap
   const int kWTap = kWPlane * planes;
   const int kTileH = prob->tile_h, kTileW = prob->tile_w;
-  constexpr int kHaloBox = halo_box_bytes(KC), kHaloPlane = halo_plane_bytes(KC), kHaloStage = halo_stage_bytes(KC);
-  const bool halo = prob->halo != 0;   // plan guarantees 16x8 tiles
+  constexpr int kHaloBox = halo_box_bytes(KC), kHaloPlane = halo_plane_bytes(KC);
+  constexpr bool halo = kHalo;   // plan guarantees 16x8 tiles
   const int kAPlane = halo ? kHaloPlane : a_plane_bytes(KC, kTileH, kTileW);
   const int kAStage = planes * kAPlane;
-  (void)kHaloStage;
   const int kRowStep = kTileW * KC * 2;  // one tile row of pixels = tile_w/8 swizzle atoms
   constexpr bool kFused = BN <= 128;
-  constexpr uint32_t kAccCols = kFused ? 2 * BN : BN;
-  constexpr uint32_t kTmemCols = 2 * kAccCols;
+  constexpr int kAccRegs = (kFused ? 2 * BN : BN) / 2;
 
   // ---- problem fields -> registers, once (the asm "memory" clobbers would otherwise force a
   //      global reload of every P.* access inside the role loops)
@@ -94,6 +90,18 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
   for (int s = 0; s < nsrc; ++s) nkb += prob->src[s].nchunk * 9;
 
   const FastDiv div_nt(n_nt, ntiles), div_img(tiles_per_img, ntiles), div_tx(tiles_x, ntiles);   // tile decode
+  // CTA pair (prob->pair, launched as (2,1,1) clusters): the two CTAs of a cluster walk the same work list, each on its
+  // own spatial tile of a neighbouring pair, with the same N tile and hence the same weight taps.  Each CTA loads half of
+  // every streamed weight tap and multicasts it into both CTAs' weight rings: half the L2 -> SM weight traffic per CTA.
+  const bool pair = prob->pair != 0;
+  const int rank = pair ? (int)cluster_ctarank() : 0;
+  const int nsp = prob->B * tiles_per_img;                      // spatial tiles
+  const int nwork = pair ? ((nsp + 1) / 2) * n_nt : ntiles;
+  const int w_first = pair ? (int)blockIdx.x >> 1 : (int)blockIdx.x, w_step = pair ? (int)gridDim.x >> 1 : (int)gridDim.x;
+  auto decode = [&](int work, int& sp, int& nti) {   // -> spatial tile (>= nsp: the empty partner of an odd count), N tile
+    div_nt.divmod(work, sp, nti);
+    if (pair) sp = 2 * sp + rank;
+  };
 
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;
@@ -103,23 +111,18 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
   const uint32_t w_bytes = resident ? (uint32_t)nkb * kWTap : (uint32_t)NW * kWTap;
   const uint32_t tail = w_base + w_bytes;
   const uint32_t tail_off = (uint32_t)NA * kAStage + w_bytes;
-  // barrier k lives at tail + 8k: a_full[0..7], a_empty[8..15], w_full[16..23], w_empty[24..31], t_full[32,33], t_empty[34,35]
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(gen_base + tail_off + kBarBytes);
+  // barrier k lives at tail + 8k: a_full[0..7], a_empty[8..15], w_full[16..23], w_empty[24..31]
   float* bias_smem = reinterpret_cast<float*>(gen_base + tail_off + kBarBytes + 16);
   int* src_tab = reinterpret_cast<int*>(gen_base + tail_off + kBarBytes + 16 + 512 * 4);  // {nchunk, c_off} x 4
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     for (int s = 0; s < kMaxRing; ++s) {
       mbar_init(tail + 8u * s, 1);
-      mbar_init(tail + 8u * (kMaxRing + s), 1);
+      mbar_init(tail + 8u * (kMaxRing + s), 2);       // one arrive per consumer warpgroup
       mbar_init(tail + 8u * (2 * kMaxRing + s), 1);
-      mbar_init(tail + 8u * (3 * kMaxRing + s), 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(tail + 8u * (4 * kMaxRing + s), 1);
-      mbar_init(tail + 8u * (4 * kMaxRing + 2 + s), kEpiWarps);  // one arrive per epilogue warp
+      mbar_init(tail + 8u * (3 * kMaxRing + s), pair ? 4 : 2);   // a pair's weight slot is free once both CTAs read it
     }
     for (int s = 0; s < kMaxSrc; ++s) {
       src_tab[2 * s] = s < nsrc ? prob->src[s].nchunk : 0;
@@ -129,15 +132,21 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_ptr_smem), kTmemCols);
-  if (warp >= 2)
-    for (int i = threadIdx.x - 64; i < n_nt * BN; i += 32 * kEpiWarps) bias_smem[i] = (i < cout) ? prob->bias[i] : 0.f;
-  tc_fence_before();
+  if (warp < 8)
+    for (int i = threadIdx.x; i < n_nt * BN; i += kConsumers) bias_smem[i] = (i < cout) ? prob->bias[i] : 0.f;
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
+  if (pair) cluster_sync_all();   // the peer's barriers are initialised before any multicast or remote arrive
+  // a CTA of a pair leaves only together with its peer: the peer's consumers still arrive on this CTA's barriers
+  auto leave = [&]() {
+    if (pair) cluster_sync_all();
+  };
 
-  if (warp == 0) {
+  if (warp >= 8) {
+    regs_dec<40>();
+    if (warp > 8) {
+      leave();
+      return;
+    }
     // ============================ TMA producer (warp-uniform) ============================
     const CUtensorMap* tm_w_hi = &prob->tm_w_hi;
     const CUtensorMap* tm_w_lo = &prob->tm_w_lo;
@@ -151,20 +160,20 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
     }
     __syncwarp();
     RingPos ra, rw;   // activation / weight ring positions
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
+    for (int tile = w_first; tile < nwork; tile += w_step) {
       int sp, nti, b, rem, ty, tx;
-      div_nt.divmod(tile, sp, nti);
-      div_img.divmod(sp, b, rem);
+      decode(tile, sp, nti);
+      div_img.divmod(sp, b, rem);   // an empty partner tile decodes to b = B: every TMA box is out of bounds (zeros)
       div_tx.divmod(rem, ty, tx);
       const int n0 = nti * BN, y0 = ty * kTileH, x0 = tx * kTileW;
       {
         // L2 prefetch of this CTA's NEXT spatial tile: first touch of an activation tile is DRAM
-        const int nt = tile + gridDim.x;
-        int nsp, nnt;
-        div_nt.divmod(nt < ntiles ? nt : 0, nsp, nnt);
-        if (nt < ntiles && nsp != sp && elect_one()) {
+        const int nt = tile + w_step;
+        int next_sp, nnt;
+        decode(nt < nwork ? nt : 0, next_sp, nnt);
+        if (nt < nwork && next_sp != sp && next_sp < nsp && elect_one()) {
           int nb, nrem, nty, ntx;
-          div_img.divmod(nsp, nb, nrem);
+          div_img.divmod(next_sp, nb, nrem);
           div_tx.divmod(nrem, nty, ntx);
           const int ny0 = nty * kTileH, nx0 = ntx * kTileW;
           for (int s = 0; s < nsrc; ++s)
@@ -208,8 +217,14 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
                 if (elect_one()) {
                   const uint32_t sw = w_base + ws * kWTap, bar = tail + 8u * (2 * kMaxRing + ws);
                   mbar_expect_tx(bar, kWTap);
-                  tma_load_2d(sw, tm_w_hi, bar, kb * KC, n0);
-                  if (!one) tma_load_2d(sw + kWPlane, tm_w_lo, bar, kb * KC, n0);
+                  if (pair) {   // this CTA's half of the tap's rows, into the same slot of both CTAs
+                    const uint32_t hoff = (uint32_t)(rank * (kWPlane / 2));
+                    tma_load_2d_mc(sw + hoff, &prob->tm_w_hi_half, bar, kb * KC, n0 + rank * (BN / 2), 3);
+                    if (!one) tma_load_2d_mc(sw + kWPlane + hoff, &prob->tm_w_lo_half, bar, kb * KC, n0 + rank * (BN / 2), 3);
+                  } else {
+                    tma_load_2d(sw, tm_w_hi, bar, kb * KC, n0);
+                    if (!one) tma_load_2d(sw + kWPlane, tm_w_lo, bar, kb * KC, n0);
+                  }
                 }
                 __syncwarp();
                 rw.advance(NW);
@@ -219,347 +234,326 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================ MMA issuer (warp-uniform, elected lane issues) ============================
-    const uint32_t idesc = make_idesc<BN>();
-    const uint32_t idesc2 = make_idesc<(kFused ? 2 * BN : BN)>();
-    if (resident) {
-      mbar_wait(tail + 8u * (2 * kMaxRing), 0);
-      tc_fence_after();
+    leave();
+    return;
+  }
+
+  // ============================ consumer warpgroups: MMA + epilogue ============================
+  regs_inc<232>();
+  const int wg = warp >> 2;        // pixels [64 wg, 64 wg + 64) of the tile
+  const int q = lane & 3;
+  const int H = prob->H, W = prob->W, out_H = prob->out_H, out_W = prob->out_W, out_C = prob->out_C;
+  const int out_c_off = prob->out_c_off, act = prob->act;
+  sp_t* const out_hi = prob->out_hi;
+  sp_t* const out_lo = prob->out_lo;
+  // fused 2x2/2 average pool: only for 16x8 tiles, where the 2x2 partners of the pixel in fragment row r0 are the
+  // same thread's row r0 + 8 (next tile row) and lane ^ 4 (next column)
+  sp_t* const pool_hi = prob->pool_hi;
+  sp_t* const pool_lo = prob->pool_lo;
+  const int pool_C = prob->pool_C;
+  const bool do_pool = pool_hi != nullptr;
+  const bool lo_skip = prob->out_lo_skip != 0;
+  // RGB-head mode: channel partial sums of the 1x1 64 -> 3 conv, reduced over the four lanes that share a pixel
+  const bool rgb = prob->epi_mode == 2;
+  const float* const head_w = prob->head_w4;
+  float* const rgb_out = prob->head_v;
+  const int crop_y = prob->crop_y, crop_x = prob->crop_x, crop_h = prob->crop_h, crop_w = prob->crop_w;
+  const int64_t crop_pitch = prob->crop_pitch;
+  // flow-head mode (BN <= 64): hidden units = BN / 2; each lane accumulates the partial sums of its channels for every
+  // hidden unit, the four lanes of a pixel combine with shuffles and finish the head
+  const bool fhead = prob->epi_mode == 3;
+  constexpr int kHid = BN <= 64 ? BN / 2 : 1;
+  float* const w3s = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(src_tab) + 64);   // [BN][kHid]
+  float* const hmisc = w3s + kHeadW3 / 4;                                                  // b3[kHid] | w4[kHid][2] | b4[2]
+  if (fhead) {
+    if constexpr (BN <= 64) {
+      for (int i = threadIdx.x; i < BN * kHid; i += kConsumers) w3s[i] = prob->head_w3[i];
+      for (int i = threadIdx.x; i < kHid; i += kConsumers) hmisc[i] = prob->head_b3[i];
+      for (int i = threadIdx.x; i < 2 * kHid; i += kConsumers) hmisc[kHid + i] = prob->head_w4[i];
+      if (threadIdx.x < 2) hmisc[3 * kHid + threadIdx.x] = prob->head_b4[threadIdx.x];
     }
-    // The item loop is instantiated twice: sources whose trailing 16-channel k-steps are zero padding in every
-    // chunk (ConvSrc::ksteps < KC/16: the 10-of-64 "side" source, the 3-of-32 image block) skip those k-steps;
-    // every other layer runs the loop without the bookkeeping (the issuing warp is issue-bound).
-    bool any_partial = false;
-    for (int s = 0; s < kMaxSrc; ++s) any_partial |= src_tab[2 * s] > 0 && src_tab[2 * kMaxSrc + s] < KC / 16;
-    // Halo mode: one activation stage per chunk carries all nine taps; tap t = 3*dx + dy (the K order of the
-    // packed weights) reads the box at byte offset (dy * 10 + dx) * 128, 8-row groups 1280 B apart.
-    auto run_items = [&](auto partial_tag, auto halo_tag, auto one_tag, auto res_tag) {
-      constexpr bool kPartial = decltype(partial_tag)::value;
-      constexpr bool kHalo = decltype(halo_tag)::value;
-      constexpr bool kOne = decltype(one_tag)::value;   // single-pass product
-      constexpr bool kRes = decltype(res_tag)::value;   // weights resident in smem: no waits between the taps of a stage
-      constexpr int kWTapC = kWPlane * (kOne ? 1 : 2);
-      constexpr int kStageTaps = kHalo ? 9 : 3;   // taps served by one activation stage
-      constexpr int kSrcStages = kHalo ? 1 : 3;   // activation stages per chunk
-      const int nab = nkb / kStageTaps;           // activation stages per tile
-      RingPos ra, rw;   // activation / weight ring positions
-      uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-        const uint32_t acc = it & 1u;
-        mbar_wait(tail + 8u * (4 * kMaxRing + 2 + acc), ((it >> 1) & 1u) ^ 1u);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * kAccCols;
-        int kb = 0;
-        [[maybe_unused]] int src_i = 0, src_left = src_tab[0] * kSrcStages;  // stages left in the current source
-        for (int ab = 0; ab < nab; ++ab) {
-          [[maybe_unused]] int ksteps = KC / 16;
-          if constexpr (kPartial) {
-            while (src_left == 0) {
-              ++src_i;
-              src_left = src_tab[2 * src_i] * kSrcStages;
-            }
-            --src_left;
-            ksteps = src_tab[2 * kMaxSrc + src_i];
+    asm volatile("bar.sync 1, %0;" ::"r"(kConsumers) : "memory");   // consumer warps only
+  }
+  const float* const head_vup = prob->head_vup;
+  float* const head_res = prob->head_res;
+  float* const head_vout = prob->head_v;
+
+  if (resident) mbar_wait(tail + 8u * (2 * kMaxRing), 0);
+  const bool is_leader = (threadIdx.x & 127) == 0;
+  const uint32_t w_empty_peer = pair ? map_to_cta(tail + 8u * (3 * kMaxRing), (uint32_t)(rank ^ 1)) : 0u;
+  auto release_w = [&](int slot) {
+    mbar_arrive(tail + 8u * (3 * kMaxRing + slot));
+    if (pair) mbar_arrive_cluster(w_empty_peer + 8u * slot);
+  };
+  {
+    constexpr int kWTapC = kWPlane * (kOne ? 1 : 2);
+    constexpr int kStageTaps = kHalo ? 9 : 3;   // taps served by one activation stage
+    constexpr int kSrcStages = kHalo ? 1 : 3;   // activation stages per chunk
+    constexpr uint32_t kPx = KC * 2;            // bytes of one pixel row of a box
+    const int nab = nkb / kStageTaps;           // activation stages per tile
+    // first pixel row of this warpgroup's 64 pixels inside the box, and the stride between its 8-row groups
+    const uint32_t a_row0 = kHalo ? (uint32_t)(wg * 8 * kHaloW) * kPx : (uint32_t)(wg * 64) * kPx;
+    const uint32_t sbo = kHalo ? kHaloW * kPx : 8 * kPx;
+    RingPos ra, rw;   // activation / weight ring positions
+    float acc[kAccRegs];
+    for (int tile = w_first; tile < nwork; tile += w_step) {
+      int kb = 0;
+      int rel_a = -1, rel_w = -1;   // stages read by the previous wgmma group, released once it retired
+      auto retire = [&](int next_a, int next_w) {
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (is_leader) {
+          if (rel_a >= 0) mbar_arrive(tail + 8u * (kMaxRing + rel_a));
+          if (rel_w >= 0) release_w(rel_w);
+        }
+        rel_a = next_a;
+        rel_w = next_w;
+      };
+      [[maybe_unused]] int src_i = 0, src_left = src_tab[0] * kSrcStages;  // stages left in the current source
+      for (int ab = 0; ab < nab; ++ab) {
+        [[maybe_unused]] int ksteps = KC / 16;
+        if constexpr (kPartial) {
+          while (src_left == 0) {
+            ++src_i;
+            src_left = src_tab[2 * src_i] * kSrcStages;
           }
-          const int st = ra.stage;
-          mbar_wait(tail + 8u * st, ra.phase);
-          tc_fence_after();
-          const uint32_t sa = a_base + st * kAStage;
-          if constexpr (kRes) {
-            // Resident weights: nothing to wait for inside the stage, so ONE elected lane issues all of its taps as
-            // straight-line code -- descriptors are a base plus compile-time offsets (the 14-bit address field
-            // cannot carry: smem offsets are < 256 KiB), ~2 instructions per MMA instead of ~90 per tap.
-            if (elect_one()) {
-              constexpr uint32_t kPx = KC * 2;   // bytes of one pixel row of the box
-              const uint64_t a0 = kHalo ? make_desc_sbo<KC>(sa, kHaloW * kPx) : make_desc_kc<KC>(sa);
-              const uint64_t lo_delta = (uint64_t)((kHalo ? kHaloPlane : kAPlane) >> 4);
-              const uint64_t row_delta = (uint64_t)(kRowStep >> 4);
-              const uint64_t w0 = make_desc_kc<KC>(w_base + kb * kWTapC);
-              const uint32_t first = (kb == 0) ? 0u : 1u;
+          --src_left;
+          ksteps = src_tab[2 * kMaxSrc + src_i];
+        }
+        const int st = ra.stage;
+        mbar_wait(tail + 8u * st, ra.phase);
+        const uint32_t sa = a_base + st * kAStage + a_row0;
+        const uint32_t lo_off = (uint32_t)(kHalo ? kHaloPlane : kAPlane);
+        if constexpr (kRes) {
+          // Resident weights: nothing to wait for inside the stage, so all of its taps are one wgmma group issued as
+          // straight-line code with compile-time descriptor offsets
+          const uint64_t a0 = make_desc_sbo<KC>(sa, sbo);
+          const uint64_t lo_delta = (uint64_t)(lo_off >> 4);
+          const uint64_t row_delta = (uint64_t)(kRowStep >> 4);
+          const uint64_t w0 = make_desc_kc<KC>(w_base + kb * kWTapC);
+          const uint32_t first = (kb == 0) ? 0u : 1u;
+          wgmma_fence();
 #pragma unroll
-              for (int t = 0; t < kStageTaps; ++t) {
-                const uint64_t a_hi = a0 + (kHalo ? (uint64_t)((((t % 3) * kHaloW + t / 3) * kPx) >> 4) : (uint64_t)t * row_delta);
-                const uint64_t a_lo = a_hi + lo_delta;
-                const uint64_t w_hi = w0 + (uint64_t)((t * kWTapC) >> 4), w_lo = w_hi + (uint64_t)(kWPlane >> 4);
+          for (int t = 0; t < kStageTaps; ++t) {
+            const uint64_t a_hi = a0 + (kHalo ? (uint64_t)((((t % 3) * kHaloW + t / 3) * kPx) >> 4) : (uint64_t)t * row_delta);
+            const uint64_t a_lo = a_hi + lo_delta;
+            const uint64_t w_hi = w0 + (uint64_t)((t * kWTapC) >> 4), w_lo = w_hi + (uint64_t)(kWPlane >> 4);
 #pragma unroll
-                for (int k = 0; k < KC / 16; ++k) {
-                  if (!kPartial || k < ksteps) {
-                    const uint64_t adv = (uint64_t)(k * 32 >> 4);
-                    const uint32_t accf = (t == 0 && k == 0) ? first : 1u;
-                    if constexpr (kOne) {
-                      umma(d_tmem, a_hi + adv, w_hi + adv, idesc, accf);
-                    } else if constexpr (kFused) {
-                      umma(d_tmem, a_hi + adv, w_hi + adv, idesc2, accf);  // N = 2*BN: [W_hi ; W_lo]
-                      umma(d_tmem, a_lo + adv, w_hi + adv, idesc, 1u);
-                    } else {
-                      umma(d_tmem, a_lo + adv, w_hi + adv, idesc, accf);
-                      umma(d_tmem, a_hi + adv, w_lo + adv, idesc, 1u);
-                      umma(d_tmem, a_hi + adv, w_hi + adv, idesc, 1u);
-                    }
-                  }
+            for (int k = 0; k < KC / 16; ++k) {
+              if (!kPartial || k < ksteps) {
+                const uint64_t adv = (uint64_t)(k * 32 >> 4);
+                const uint32_t accf = (t == 0 && k == 0) ? first : 1u;
+                if constexpr (kOne) {
+                  wgmma<BN>(acc, a_hi + adv, w_hi + adv, accf);
+                } else if constexpr (kFused) {
+                  wgmma<BN>(acc, a_hi + adv, w_hi + adv, accf);
+                  wgmma<BN>(acc + BN / 2, a_hi + adv, w_lo + adv, accf);
+                  wgmma<BN>(acc, a_lo + adv, w_hi + adv, 1u);
+                } else {
+                  wgmma<BN>(acc, a_lo + adv, w_hi + adv, accf);
+                  wgmma<BN>(acc, a_hi + adv, w_lo + adv, 1u);
+                  wgmma<BN>(acc, a_hi + adv, w_hi + adv, 1u);
                 }
               }
-              umma_commit(tail + 8u * (kMaxRing + st));
-              if (ab == nab - 1) umma_commit(tail + 8u * (4 * kMaxRing + acc));
             }
-            __syncwarp();
-            kb += kStageTaps;
-          } else {
+          }
+          retire(st, -1);
+          kb += kStageTaps;
+        } else {
           for (int t = 0; t < kStageTaps; ++t, ++kb) {
             uint32_t sw;
-            int ws = 0;
+            int ws = -1;
             if (resident) {
               sw = w_base + kb * kWTap;
             } else {
               ws = rw.stage;
               mbar_wait(tail + 8u * (2 * kMaxRing + ws), rw.phase);
-              tc_fence_after();
               sw = w_base + ws * kWTap;
             }
-            if (elect_one()) {
-              uint64_t a_hi, a_lo;
-              if constexpr (kHalo) {
-                constexpr uint32_t kPx = KC * 2;   // bytes of one pixel row of the box
-                const uint32_t off = (uint32_t)((t % 3) * kHaloW + t / 3) * kPx;
-                a_hi = make_desc_sbo<KC>(sa + off, kHaloW * kPx);
-                a_lo = make_desc_sbo<KC>(sa + kHaloPlane + off, kHaloW * kPx);
+            const uint32_t off = kHalo ? (uint32_t)((t % 3) * kHaloW + t / 3) * kPx : (uint32_t)(t * kRowStep);
+            const uint64_t a_hi = make_desc_sbo<KC>(sa + off, sbo);
+            const uint64_t a_lo = make_desc_sbo<KC>(sa + lo_off + off, sbo);
+            const uint64_t w_hi = make_desc_kc<KC>(sw), w_lo = make_desc_kc<KC>(sw + kWPlane);
+            const uint32_t first = (kb == 0) ? 0u : 1u;
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < KC / 16; ++k) {
+              if constexpr (kPartial) {
+                if (k >= ksteps) break;
+              }
+              const uint64_t adv = (uint64_t)(k * 32 >> 4);
+              if constexpr (kOne) {
+                wgmma<BN>(acc, a_hi + adv, w_hi + adv, k == 0 ? first : 1u);
+              } else if constexpr (kFused) {
+                wgmma<BN>(acc, a_hi + adv, w_hi + adv, k == 0 ? first : 1u);
+                wgmma<BN>(acc + BN / 2, a_hi + adv, w_lo + adv, k == 0 ? first : 1u);
+                wgmma<BN>(acc, a_lo + adv, w_hi + adv, 1u);
               } else {
-                a_hi = make_desc_kc<KC>(sa + t * kRowStep);
-                a_lo = make_desc_kc<KC>(sa + kAPlane + t * kRowStep);
+                wgmma<BN>(acc, a_lo + adv, w_hi + adv, k == 0 ? first : 1u);
+                wgmma<BN>(acc, a_hi + adv, w_lo + adv, 1u);
+                wgmma<BN>(acc, a_hi + adv, w_hi + adv, 1u);
               }
-              const uint64_t w_hi = make_desc_kc<KC>(sw), w_lo = make_desc_kc<KC>(sw + kWPlane);
-              const uint32_t first = (kb == 0) ? 0u : 1u;
-  #pragma unroll
-              for (int k = 0; k < KC / 16; ++k) {
-                if constexpr (kPartial) {
-                  if (k >= ksteps) break;
-                }
-                const uint64_t adv = (uint64_t)(k * 32 >> 4);
-                if constexpr (kOne) {
-                  umma(d_tmem, a_hi + adv, w_hi + adv, idesc, k == 0 ? first : 1u);
-                } else if constexpr (kFused) {
-                  umma(d_tmem, a_hi + adv, w_hi + adv, idesc2, k == 0 ? first : 1u);  // N = 2*BN: [W_hi ; W_lo]
-                  umma(d_tmem, a_lo + adv, w_hi + adv, idesc, 1u);
-                } else {
-                  umma(d_tmem, a_lo + adv, w_hi + adv, idesc, k == 0 ? first : 1u);
-                  umma(d_tmem, a_hi + adv, w_lo + adv, idesc, 1u);
-                  umma(d_tmem, a_hi + adv, w_hi + adv, idesc, 1u);
-                }
-              }
-              if (!resident) umma_commit(tail + 8u * (3 * kMaxRing + ws));
-              if (t == kStageTaps - 1) umma_commit(tail + 8u * (kMaxRing + st));
-              if (t == kStageTaps - 1 && ab == nab - 1) umma_commit(tail + 8u * (4 * kMaxRing + acc));
             }
-            __syncwarp();
+            retire(t == kStageTaps - 1 ? st : -1, ws);
             if (!resident) rw.advance(NW);
           }
-          }  // per-tap issue loop
-          ra.advance(NA);
         }
+        ra.advance(NA);
       }
-    };
-    auto run_pass = [&](auto one_tag, auto res_tag) {
-      if (halo) {
-        if (any_partial) run_items(std::true_type{}, std::true_type{}, one_tag, res_tag);
-        else run_items(std::false_type{}, std::true_type{}, one_tag, res_tag);
-      } else {
-        if (any_partial) run_items(std::true_type{}, std::false_type{}, one_tag, res_tag);
-        else run_items(std::false_type{}, std::false_type{}, one_tag, res_tag);
+      wgmma_wait<0>();
+      if (is_leader) {
+        if (rel_a >= 0) mbar_arrive(tail + 8u * (kMaxRing + rel_a));
+        if (rel_w >= 0) release_w(rel_w);
       }
-    };
-    if (resident && prob->straight) {
-      if (one) run_pass(std::true_type{}, std::true_type{});
-      else run_pass(std::false_type{}, std::true_type{});
-    } else {
-      if (one) run_pass(std::true_type{}, std::false_type{});
-      else run_pass(std::false_type{}, std::false_type{});
-    }
-  } else {
-    // ============================ epilogue (warps 2..9) ============================
-    const int q = warp & 3;              // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;    // which 16-column chunks (even / odd) this warp drains
-    const int r = q * 32 + lane;
-    const int r_y = r / kTileW, r_x = r % kTileW;   // position of this thread's pixel inside the tile (tile-invariant)
-    const int H = prob->H, W = prob->W, out_H = prob->out_H, out_W = prob->out_W, out_C = prob->out_C;
-    const int out_c_off = prob->out_c_off, act = prob->act;
-    sp_t* const out_hi = prob->out_hi;
-    sp_t* const out_lo = prob->out_lo;
-    // fused 2x2/2 average pool: only for 16x8 tiles (a warp's 32 lanes = 4 tile rows x 8 columns, so
-    // the 2x2 partners of lane l are l^1, l^8, l^9 -> three warp shuffles on the fp32 values)
-    sp_t* const pool_hi = prob->pool_hi;
-    sp_t* const pool_lo = prob->pool_lo;
-    const int pool_C = prob->pool_C;
-    const bool do_pool = pool_hi != nullptr;
-    const bool lo_skip = prob->out_lo_skip != 0;
-    // RGB-head mode: channel partial sums of the 1x1 64 -> 3 conv; the two warps of a lane quarter own 32 channels each
-    // and combine through shared memory (named barrier per quarter)
-    const bool rgb = prob->epi_mode == 2;
-    const float* const head_w = prob->head_w4;
-    float* const rgb_out = prob->head_v;
-    const int crop_y = prob->crop_y, crop_x = prob->crop_x, crop_h = prob->crop_h, crop_w = prob->crop_w;
-    const int64_t crop_pitch = prob->crop_pitch;
-    float* const part = bias_smem + 64;   // [128 rows][3] (bias_smem holds 64 biases in this mode, 512 floats in all)
-    // flow-head mode (BN <= 64): hidden units = BN / 2; each warp of a lane quarter accumulates the partial sums of its
-    // channels for every hidden unit, the pair combines through smem ([hidden][row]: conflict-free) and finishes the head
-    const bool fhead = prob->epi_mode == 3;
-    constexpr int kHid = BN <= 64 ? BN / 2 : 1;
-    float* const hpart = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(src_tab) + 64);   // [kHid][128]
-    float* const w3s = hpart + kHeadPart / 4;                                                   // [BN][kHid]
-    float* const hmisc = w3s + kHeadW3 / 4;                                                     // b3[kHid] | w4[kHid][2] | b4[2]
-    if (fhead) {
-      if constexpr (BN <= 64) {
-        for (int i = threadIdx.x - 64; i < BN * kHid; i += 32 * kEpiWarps) w3s[i] = prob->head_w3[i];
-        for (int i = threadIdx.x - 64; i < kHid; i += 32 * kEpiWarps) hmisc[i] = prob->head_b3[i];
-        for (int i = threadIdx.x - 64; i < 2 * kHid; i += 32 * kEpiWarps) hmisc[kHid + i] = prob->head_w4[i];
-        if (threadIdx.x - 64 < 2) hmisc[3 * kHid + threadIdx.x - 64] = prob->head_b4[threadIdx.x - 64];
-      }
-      asm volatile("bar.sync 5, %0;" ::"r"(32 * kEpiWarps) : "memory");   // epilogue warps only
-    }
-    const float* const head_vup = prob->head_vup;
-    float* const head_res = prob->head_res;
-    float* const head_vout = prob->head_v;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < ntiles; tile += gridDim.x, ++it) {
-      const uint32_t acc = it & 1u;
+      acc_fence<kAccRegs>(acc);
+
+      // ---------------- epilogue from the registers ----------------
       int sp, nti, b, rem, ty, tx;
-      div_nt.divmod(tile, sp, nti);
+      decode(tile, sp, nti);
       div_img.divmod(sp, b, rem);
       div_tx.divmod(rem, ty, tx);
       const int n0 = nti * BN;
-      const int py = ty * kTileH + r_y, px = tx * kTileW + r_x;
-      const bool valid = (py < H) && (px < W);
-      const int64_t opix = ((int64_t)b * out_H + py) * out_W + px;
-      sp_t* oh = out_hi + opix * out_C + out_c_off + n0;
-      sp_t* ol = out_lo + opix * out_C + out_c_off + n0;
-      mbar_wait(tail + 8u * (4 * kMaxRing + acc), (it >> 1) & 1u);
-      tc_fence_after();
-      const uint32_t t_addr = tmem_base + acc * kAccCols + ((uint32_t)(q * 32) << 16);
-      float r0 = 0.f, r1 = 0.f, r2 = 0.f;
-      [[maybe_unused]] float hp[kHid];
-      if constexpr (BN <= 64) {
+      const bool live = sp < nsp;   // false: the empty partner of an odd tile count stores nothing
+      auto value = [&](int h, int j, int e) {
+        const int i = 4 * j + 2 * h + e;
+        return (kFused && !kOne) ? acc[i] + acc[(i + BN / 2) % kAccRegs] : acc[i];
+      };
+      // RGB / flow heads: one fragment row (pixel) at a time
 #pragma unroll
-        for (int hh = 0; hh < kHid; ++hh) hp[hh] = 0.f;
-      }
-#pragma unroll 1
-      for (int cc = half; cc < BN / 16; cc += 2) {
-        if (n0 + cc * 16 >= cout) break;
-        uint32_t v[16];
-        tmem_ld16(t_addr + (uint32_t)(cc * 16), v);
-        if (kFused && !one) {
-          uint32_t u[16];
-          tmem_ld16(t_addr + (uint32_t)(BN + cc * 16), u);
-          tmem_ld_wait();
+      for (int h = 0; h < 2 && (fhead || rgb); ++h) {
+        const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+        const int py = ty * kTileH + r / kTileW, px = tx * kTileW + r % kTileW;
+        const bool valid = live && (py < H) && (px < W);
+        const int64_t opix = ((int64_t)b * out_H + py) * out_W + px;
+        if (fhead) {
+          if constexpr (BN <= 64) {
+            float hp[kHid];
 #pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(u[j]));
-        } else {
-          tmem_ld_wait();
-        }
-        {
-          float f[16];
+            for (int hh = 0; hh < kHid; ++hh) hp[hh] = 0.f;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float x = __uint_as_float(v[j]) + bias_smem[n0 + cc * 16 + j];
-            f[j] = act ? leaky(x) : x;
-          }
-          if (fhead) {
-            if constexpr (BN <= 64) {
+            for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                const float4* wr = reinterpret_cast<const float4*>(w3s + (cc * 16 + j) * kHid);   // broadcast reads
+              for (int e = 0; e < 2; ++e) {
+                const int c = 8 * j + 2 * q + e;
+                const float x = value(h, j, e) + bias_smem[n0 + c];
+                const float f = act ? leaky(x) : x;
+                const float4* wr = reinterpret_cast<const float4*>(w3s + c * kHid);
 #pragma unroll
                 for (int h4 = 0; h4 < kHid / 4; ++h4) {
                   const float4 wv = wr[h4];
-                  hp[4 * h4] = fmaf(f[j], wv.x, hp[4 * h4]);
-                  hp[4 * h4 + 1] = fmaf(f[j], wv.y, hp[4 * h4 + 1]);
-                  hp[4 * h4 + 2] = fmaf(f[j], wv.z, hp[4 * h4 + 2]);
-                  hp[4 * h4 + 3] = fmaf(f[j], wv.w, hp[4 * h4 + 3]);
+                  hp[4 * h4] = fmaf(f, wv.x, hp[4 * h4]);
+                  hp[4 * h4 + 1] = fmaf(f, wv.y, hp[4 * h4 + 1]);
+                  hp[4 * h4 + 2] = fmaf(f, wv.z, hp[4 * h4 + 2]);
+                  hp[4 * h4 + 3] = fmaf(f, wv.w, hp[4 * h4 + 3]);
                 }
               }
-            }
-          } else if (rgb) {
-            const float* hw = head_w + (n0 + cc * 16) * 3;
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              r0 = fmaf(f[j], __ldg(hw + 3 * j), r0);
-              r1 = fmaf(f[j], __ldg(hw + 3 * j + 1), r1);
-              r2 = fmaf(f[j], __ldg(hw + 3 * j + 2), r2);
+            for (int hh = 0; hh < kHid; ++hh) {
+              hp[hh] += __shfl_xor_sync(0xffffffffu, hp[hh], 1);
+              hp[hh] += __shfl_xor_sync(0xffffffffu, hp[hh], 2);
             }
-          } else if (valid) {
-            if (lo_skip) pack_store16_hi(f, oh + cc * 16);
-            else pack_store16(f, oh + cc * 16, ol + cc * 16);   // two 32-byte stores
+            if (q == 0 && valid) {
+              float f0 = hmisc[3 * kHid], f1 = hmisc[3 * kHid + 1];
+#pragma unroll
+              for (int hh = 0; hh < kHid; ++hh) {
+                const float x = leaky(hp[hh] + hmisc[hh]);       // conv_3: bias + LeakyReLU
+                f0 = fmaf(x, hmisc[kHid + 2 * hh], f0);            // conv_4: linear
+                f1 = fmaf(x, hmisc[kHid + 2 * hh + 1], f1);
+              }
+              float2 res = make_float2(f0, f1), tot = res;
+              if (head_vup) {
+                const float2 u = reinterpret_cast<const float2*>(head_vup)[opix];
+                tot.x += u.x;
+                tot.y += u.y;
+              }
+              reinterpret_cast<float2*>(head_res)[opix] = res;
+              reinterpret_cast<float2*>(head_vout)[opix] = tot;
+            }
           }
-          if (do_pool) {
-            float pf[16];
+        } else if (rgb) {
+          float r0 = 0.f, r1 = 0.f, r2 = 0.f;
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              const float a = f[j] + __shfl_xor_sync(0xffffffffu, f[j], 1);
-              pf[j] = (a + __shfl_xor_sync(0xffffffffu, a, 8)) * 0.25f;
+          for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int c = n0 + 8 * j + 2 * q + e;
+              float f = value(h, j, e) + bias_smem[c];
+              if (act) f = leaky(f);
+              r0 = fmaf(f, __ldg(head_w + 3 * c), r0);
+              r1 = fmaf(f, __ldg(head_w + 3 * c + 1), r1);
+              r2 = fmaf(f, __ldg(head_w + 3 * c + 2), r2);
             }
-            // lanes with even tile row and even tile column own the pooled pixel (H, W are even)
-            if (valid && !(lane & 1) && !(lane & 8)) {
-              const int64_t ppix = ((int64_t)b * (out_H >> 1) + (py >> 1)) * (out_W >> 1) + (px >> 1);
-              pack_store16(pf, pool_hi + ppix * pool_C + n0 + cc * 16, pool_lo + ppix * pool_C + n0 + cc * 16);
-            }
+#pragma unroll
+          for (int m = 1; m <= 2; m <<= 1) {
+            r0 += __shfl_xor_sync(0xffffffffu, r0, m);
+            r1 += __shfl_xor_sync(0xffffffffu, r1, m);
+            r2 += __shfl_xor_sync(0xffffffffu, r2, m);
+          }
+          const int oy = py - crop_y, ox = px - crop_x;
+          if (q == 0 && valid && oy >= 0 && oy < crop_h && ox >= 0 && ox < crop_w) {
+            float* o = rgb_out + (int64_t)oy * crop_pitch + (int64_t)ox * 3;
+            o[0] = r0 + __ldg(prob->head_b4);
+            o[1] = r1 + __ldg(prob->head_b4 + 1);
+            o[2] = r2 + __ldg(prob->head_b4 + 2);
           }
         }
       }
-      // accumulator drained: hand the TMEM buffer back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tail + 8u * (4 * kMaxRing + 2 + acc));
-      if (fhead) {
-        if constexpr (BN <= 64) {
-          if (half == 1) {
+      if (!fhead && !rgb) {
+        // split stores, channel block outermost: both fragment rows of a block are at hand together, so the fused pool
+        // combines tile rows y (r0) and y + 1 (r0 + 8) without holding a whole row of partial sums
+        bool valid[2];
+        int64_t opix[2];
 #pragma unroll
-            for (int hh = 0; hh < kHid; ++hh) hpart[hh * 128 + r] = hp[hh];
-          }
-          asm volatile("bar.sync %0, 64;" ::"r"(1 + q) : "memory");
-          if (half == 0 && valid) {
-            float f0 = hmisc[3 * kHid], f1 = hmisc[3 * kHid + 1];
+        for (int h = 0; h < 2; ++h) {
+          const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+          const int py = ty * kTileH + r / kTileW, px = tx * kTileW + r % kTileW;
+          valid[h] = live && (py < H) && (px < W);
+          opix[h] = ((int64_t)b * out_H + py) * out_W + px;
+        }
+        // the lane with the even tile column of row r0 owns the pooled pixel (H, W are even; pool implies 16x8 tiles)
+        const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int64_t ppix = ((int64_t)b * (out_H >> 1) + ((ty * kTileH + r0 / kTileW) >> 1)) * (out_W >> 1) +
+                             ((tx * kTileW + r0 % kTileW) >> 1);
 #pragma unroll
-            for (int hh = 0; hh < kHid; ++hh) {
-              const float x = leaky(hp[hh] + hpart[hh * 128 + r] + hmisc[hh]);     // conv_3: bias + LeakyReLU
-              f0 = fmaf(x, hmisc[kHid + 2 * hh], f0);                                  // conv_4: linear
-              f1 = fmaf(x, hmisc[kHid + 2 * hh + 1], f1);
+        for (int j = 0; j < BN / 8; ++j) {
+          const int c = 8 * j + 2 * q;
+          if (n0 + c >= cout) break;
+          float a[2][2];
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            float f0 = value(h, j, 0) + bias_smem[n0 + c], f1 = value(h, j, 1) + bias_smem[n0 + c + 1];
+            if (act) {
+              f0 = leaky(f0);
+              f1 = leaky(f1);
             }
-            float2 res = make_float2(f0, f1), tot = res;
-            if (head_vup) {
-              const float2 u = reinterpret_cast<const float2*>(head_vup)[opix];
-              tot.x += u.x;
-              tot.y += u.y;
+            if (valid[h]) {
+              sp_t* oh = out_hi + opix[h] * out_C + out_c_off + n0;
+              if (lo_skip) {
+                *reinterpret_cast<uint32_t*>(oh + c) = pack2_hi(f0, f1);
+              } else {
+                sp_t* ol = out_lo + opix[h] * out_C + out_c_off + n0;
+                uint32_t hi, lo;
+                split_pack2(f0, f1, hi, lo);
+                *reinterpret_cast<uint32_t*>(oh + c) = hi;
+                *reinterpret_cast<uint32_t*>(ol + c) = lo;
+              }
             }
-            reinterpret_cast<float2*>(head_res)[opix] = res;
-            reinterpret_cast<float2*>(head_vout)[opix] = tot;
+            if (do_pool) {   // x-pair sums: the next tile column is lane ^ 4
+              a[h][0] = f0 + __shfl_xor_sync(0xffffffffu, f0, 4);
+              a[h][1] = f1 + __shfl_xor_sync(0xffffffffu, f1, 4);
+            }
           }
-          asm volatile("bar.sync %0, 64;" ::"r"(1 + q) : "memory");   // hpart[] is rewritten by the next tile
-        }
-      } else if (rgb) {
-        if (half == 1) {
-          part[r * 3] = r0;
-          part[r * 3 + 1] = r1;
-          part[r * 3 + 2] = r2;
-        }
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + q) : "memory");
-        if (half == 0) {
-          const int oy = py - crop_y, ox = px - crop_x;
-          if (valid && oy >= 0 && oy < crop_h && ox >= 0 && ox < crop_w) {
-            float* o = rgb_out + (int64_t)oy * crop_pitch + (int64_t)ox * 3;
-            o[0] = r0 + part[r * 3] + __ldg(prob->head_b4);
-            o[1] = r1 + part[r * 3 + 1] + __ldg(prob->head_b4 + 1);
-            o[2] = r2 + part[r * 3 + 2] + __ldg(prob->head_b4 + 2);
+          if (do_pool && valid[0] && !(lane & 4)) {
+            uint32_t hi, lo;
+            split_pack2((a[0][0] + a[1][0]) * 0.25f, (a[0][1] + a[1][1]) * 0.25f, hi, lo);
+            *reinterpret_cast<uint32_t*>(pool_hi + ppix * pool_C + n0 + c) = hi;
+            *reinterpret_cast<uint32_t*>(pool_lo + ppix * pool_C + n0 + c) = lo;
           }
         }
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + q) : "memory");   // part[] is rewritten by the next tile
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
+  leave();
 }
 
 int smem_bytes_for(const ConvProblem& h, int bn) {
@@ -574,14 +568,51 @@ int smem_bytes_for(const ConvProblem& h, int bn) {
 
 int conv_tc_block_n(int cout);
 
-// Tile shape: fewest waves over the SMs first (a 151st tile costs a whole extra wave on a small
-// level), then the smallest halo.  16x8 is required by the fused pool.
-void conv3x3_tc_pick_tile(int H, int W, int B, int cout, int num_sms, int& tile_h, int& tile_w) {
+namespace {
+// Resident or streamed weights and the ring depths for one tile shape.  A consumer warpgroup releases a stage only once
+// the wgmma group AFTER the one that read it has been committed, and that group reads the next stage of the same
+// ring: both rings therefore need at least two slots, or producer and consumers wait on each other forever.
+// Returns false when the shape cannot get them within the shared-memory budget.
+bool ring_depths(int kc, int tile_h, int tile_w, int halo, int planes, int bn, int cout, int ktot, int epi_mode,
+                 int& resident, int& na, int& nw) {
+  const int wtap = w_tap_bytes(bn, kc, planes);
+  const int w_all = (ktot / kc) * wtap;
+  const int kLimit = kSmemLimit - (epi_mode == 3 ? kHeadBytes : 0);   // flow-head epilogue scratch
+  const int kAStage = a_stage_bytes_h(kc, tile_h, tile_w, halo, planes);
+  if (cout <= bn && w_all + 2 * kAStage + kFixedBytes <= kLimit) {
+    resident = 1;
+    const int n = (kLimit - kFixedBytes - w_all) / kAStage;
+    const int n_max = halo ? 3 : 6;
+    na = n > n_max ? n_max : n;
+    nw = 1;
+    return true;
+  }
+  resident = 0;
+  na = halo ? 2 : (bn >= 128 ? 2 : 3);
+  int n = (kLimit - kFixedBytes - na * kAStage) / wtap;
+  if (n < 2 && na > 2) {   // a deeper weight ring matters more than a third activation stage
+    na = 2;
+    n = (kLimit - kFixedBytes - na * kAStage) / wtap;
+  }
+  nw = n > kMaxRing ? kMaxRing : n;
+  return nw >= 2;
+}
+}  // namespace
+
+// Tile shape: fewest waves over the SMs first (a 133rd tile costs a whole extra wave on a small
+// level), then the smallest halo.  16x8 is required by the fused pool; a shape whose rings do not fit
+// (ring_depths) is never picked.
+void conv3x3_tc_pick_tile(int H, int W, int B, int cout, int kc, int passes, int ktot, int epi_mode, int num_sms,
+                          int& tile_h, int& tile_w) {
   static const int cand[3][2] = {{16, 8}, {8, 16}, {4, 32}};
-  const int bn = conv_tc_block_n(cout);
+  const int bn = conv_tc_block_n(cout);   // the engine only ever lowers BN from here, which only shrinks the rings
   const int n_nt = (cout + bn - 1) / bn;
   double best = 1e30;
+  tile_h = 16;
+  tile_w = 8;
   for (auto& c : cand) {
+    int res, na, nw;
+    if (!ring_depths(kc, c[0], c[1], 0, passes == 1 ? 1 : 2, bn, cout, ktot, epi_mode, res, na, nw)) continue;
     const long tiles = (long)B * ((H + c[0] - 1) / c[0]) * ((W + c[1] - 1) / c[1]) * n_nt;
     const long waves = (tiles + num_sms - 1) / num_sms;
     const double cost = (double)waves * (c[0] + 2.0) / c[0] * (1.0 + 1e-3 * (c[1] / 8));
@@ -593,41 +624,84 @@ void conv3x3_tc_pick_tile(int H, int W, int B, int cout, int num_sms, int& tile_
   }
 }
 
-// Chooses resident/streamed weights and the ring depths for one 3x3 problem.
-void conv3x3_tc_plan(ConvProblem& h, int num_sms) {
+// Chooses resident/streamed weights and the ring depths for one 3x3 problem; false if its rings cannot fit.
+bool conv3x3_tc_plan(ConvProblem& h, int num_sms) {
   const int bn = h.bn;
-  const int nkb = h.ktot / h.kchunk;
   const int planes = h.passes == 1 ? 1 : 2;
   const int wtap = w_tap_bytes(bn, h.kchunk, planes);
-  const int w_all = nkb * wtap;
+  const int w_all = (h.ktot / h.kchunk) * wtap;
   const bool can_resident = h.cout <= bn;
-  const int kLimit = kSmemLimit - (h.epi_mode == 3 ? kHeadBytes : 0);   // flow-head epilogue scratch
+  const int kLimit = kSmemLimit - (h.epi_mode == 3 ? kHeadBytes : 0);
   // wide halo (the engine allows it per chunk size): 16x8 tiles only; resident weights win when both do not fit
   if (h.halo && (h.tile_h != 16 || h.tile_w != 8 ||
                  (can_resident && w_all + 2 * a_stage_bytes_h(h.kchunk, h.tile_h, h.tile_w, 0, planes) + kFixedBytes <= kLimit &&
                   w_all + 2 * a_stage_bytes_h(h.kchunk, h.tile_h, h.tile_w, 1, planes) + kFixedBytes > kLimit)))
     h.halo = 0;
-  const int kAStage = a_stage_bytes_h(h.kchunk, h.tile_h, h.tile_w, h.halo, planes);
-  h.v2_resident = 0;
-  if (can_resident && w_all + 2 * kAStage + kFixedBytes <= kLimit) {
-    h.v2_resident = 1;
-    int na = (kLimit - kFixedBytes - w_all) / kAStage;
-    const int na_max = h.halo ? 3 : 6;
-    h.v2_na = na > na_max ? na_max : na;
-    h.v2_nw = 1;
-  } else {
-    h.v2_na = h.halo ? 2 : (bn >= 128 ? 2 : 3);
-    int nw = (kLimit - kFixedBytes - h.v2_na * kAStage) / wtap;
-    h.v2_nw = nw > kMaxRing ? kMaxRing : nw;
+  bool ok = ring_depths(h.kchunk, h.tile_h, h.tile_w, h.halo, planes, bn, h.cout, h.ktot, h.epi_mode, h.v2_resident,
+                        h.v2_na, h.v2_nw);
+  if (!ok && h.halo) {
+    h.halo = 0;
+    ok = ring_depths(h.kchunk, h.tile_h, h.tile_w, 0, planes, bn, h.cout, h.ktot, h.epi_mode, h.v2_resident, h.v2_na,
+                     h.v2_nw);
   }
-  const int ntiles = h.B * h.tiles_y * h.tiles_x * ((h.cout + bn - 1) / bn);
-  h.v2_grid = ntiles < num_sms ? ntiles : num_sms;
+  const int nsp = h.B * h.tiles_y * h.tiles_x, n_nt = (h.cout + bn - 1) / bn;
+  if (h.pair) {   // (2,1,1) clusters, one work item = a pair of spatial tiles
+    const int nwork = (nsp + 1) / 2 * n_nt, nclu = num_sms / 2;
+    h.v2_grid = 2 * (nwork < nclu ? nwork : nclu);
+  } else {
+    h.v2_grid = nsp * n_nt < num_sms ? nsp * n_nt : num_sms;
+  }
+  return ok;
 }
+
+template <int BN, int KC>
+struct Variants {
+  // every (kPartial, kHalo, kOne, kRes) instantiation of one (BN, KC) kernel, indexed by the four bits
+  static constexpr void (*kFn[16])(const ConvProblem*) = {
+      k_conv3x3_tc<BN, KC, false, false, false, false>, k_conv3x3_tc<BN, KC, false, false, false, true>,
+      k_conv3x3_tc<BN, KC, false, false, true, false>,  k_conv3x3_tc<BN, KC, false, false, true, true>,
+      k_conv3x3_tc<BN, KC, false, true, false, false>,  k_conv3x3_tc<BN, KC, false, true, false, true>,
+      k_conv3x3_tc<BN, KC, false, true, true, false>,   k_conv3x3_tc<BN, KC, false, true, true, true>,
+      k_conv3x3_tc<BN, KC, true, false, false, false>,  k_conv3x3_tc<BN, KC, true, false, false, true>,
+      k_conv3x3_tc<BN, KC, true, false, true, false>,   k_conv3x3_tc<BN, KC, true, false, true, true>,
+      k_conv3x3_tc<BN, KC, true, true, false, false>,   k_conv3x3_tc<BN, KC, true, true, false, true>,
+      k_conv3x3_tc<BN, KC, true, true, true, false>,    k_conv3x3_tc<BN, KC, true, true, true, true>};
+  static cudaError_t configure() {
+    for (auto fn : kFn) {
+      const cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
+      if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+  }
+  static cudaError_t launch(const ConvProblem* d_prob, const ConvProblem& h, cudaStream_t st) {
+    if (h.v2_na < 2 || (!h.v2_resident && h.v2_nw < 2)) return cudaErrorInvalidValue;   // see ring_depths
+    bool partial = false;
+    for (int s = 0; s < h.nsrc; ++s) partial |= h.src[s].nchunk > 0 && h.src[s].ksteps < KC / 16;
+    const int idx = (partial ? 8 : 0) | (h.halo ? 4 : 0) | (h.passes == 1 ? 2 : 0) | (h.v2_resident && h.straight ? 1 : 0);
+    if (!h.pair) {
+      kFn[idx]<<<h.v2_grid, kThreads, smem_bytes_for(h, BN), st>>>(d_prob);
+      return cudaGetLastError();
+    }
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.gridDim = dim3(h.v2_grid);
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = smem_bytes_for(h, BN);
+    cfg.stream = st;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, kFn[idx], d_prob);
+  }
+};
 
 cudaError_t conv3x3_tc_configure() {
   cudaError_t e;
-#define FILM_CFG(BN, KC)                                                                                     \
-  e = cudaFuncSetAttribute(k_conv3x3_tc<BN, KC>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);   \
+#define FILM_CFG(BN, KC)                        \
+  e = Variants<BN, KC>::configure();            \
   if (e != cudaSuccess) return e;
   FILM_CFG(32, 64) FILM_CFG(64, 64) FILM_CFG(128, 64) FILM_CFG(256, 64) FILM_CFG(32, 32) FILM_CFG(64, 32)
 #undef FILM_CFG
@@ -636,20 +710,17 @@ cudaError_t conv3x3_tc_configure() {
 
 cudaError_t launch_conv3x3_tc(const ConvProblem* d_prob, const ConvProblem& h, cudaStream_t st) {
   const int bn = h.bn;
-  const int smem = smem_bytes_for(h, bn);
   if (h.kchunk == 32) {  // 32-channel K blocks: the 32 -> 32 flow convs and the 3(32) -> 64 first conv
-    if (bn == 32) k_conv3x3_tc<32, 32><<<h.v2_grid, kThreads, smem, st>>>(d_prob);
-    else if (bn == 64) k_conv3x3_tc<64, 32><<<h.v2_grid, kThreads, smem, st>>>(d_prob);
-    else return cudaErrorInvalidValue;
-    return cudaGetLastError();
+    if (bn == 32) return Variants<32, 32>::launch(d_prob, h, st);
+    if (bn == 64) return Variants<64, 32>::launch(d_prob, h, st);
+    return cudaErrorInvalidValue;
   }
   switch (bn) {
-    case 256: k_conv3x3_tc<256, 64><<<h.v2_grid, kThreads, smem, st>>>(d_prob); break;
-    case 128: k_conv3x3_tc<128, 64><<<h.v2_grid, kThreads, smem, st>>>(d_prob); break;
-    case 64: k_conv3x3_tc<64, 64><<<h.v2_grid, kThreads, smem, st>>>(d_prob); break;
-    default: k_conv3x3_tc<32, 64><<<h.v2_grid, kThreads, smem, st>>>(d_prob); break;
+    case 256: return Variants<256, 64>::launch(d_prob, h, st);
+    case 128: return Variants<128, 64>::launch(d_prob, h, st);
+    case 64: return Variants<64, 64>::launch(d_prob, h, st);
+    default: return Variants<32, 64>::launch(d_prob, h, st);
   }
-  return cudaGetLastError();
 }
 
 }  // namespace film

@@ -1,25 +1,22 @@
-// tcgen05 implicit-GEMM convolution for sm_100a (the engine's hot kernel).
+// wgmma implicit-GEMM convolution for sm_90a (the engine's generic tensor-core kernel).
 //
 // One CTA computes a 128-pixel (tile_h x tile_w) x BN-channel output tile of one Conv2D
 // call site (film_conv.h).  GEMM view: D[128 x BN] += A[128 x 64] * W[BN x 64]^T per K block,
 // K blocks = (source, 64-channel chunk, tap).
 //
-//   warp 0    : TMA producer.  Per K block: 4-D tiled TMA loads of the hi and lo planes of the
-//               activation box (64 ch, tile_w, tile_h, 1) at the tap-shifted coordinate --
-//               out-of-bounds rows/cols are zero-filled by TMA, which IS the SAME padding of
-//               tf.keras Conv2D -- plus 2-D loads of the W_hi / W_lo [BN x 64] blocks.
-//               Everything lands in SWIZZLE_128B K-major layout (one pixel = one 128 B row).
-//   warp 1    : allocates TMEM (BN fp32 columns) and issues tcgen05.mma.kind::f16 (M=128,
-//               N=BN, K=16): per K block 4 k-steps x 3 passes  A_hi*W_hi + A_hi*W_lo + A_lo*W_hi
-//               (split-precision product, fp32 accumulate in TMEM).  tcgen05.commit releases
-//               smem stages back to the producer and finally signals the epilogue.
-//   warps 2-5 : epilogue.  tcgen05.ld (32 lanes x 32 columns per warp), + bias, LeakyReLU,
-//               re-split to hi/lo 16-bit planes, 128-bit stores into the destination channel
-//               slice (which is how channel concats and the NN-upsample parity scatter are
-//               realised without extra passes).
+//   warp 8     : TMA producer (warpgroup 2; its registers are handed to the consumers).  Per K block: 4-D tiled
+//                TMA loads of the hi and lo planes of the activation box (64 ch, tile_w, tile_h, 1) at the tap-shifted coordinate --
+//                out-of-bounds rows/cols are zero-filled by TMA, which IS the SAME padding of
+//                tf.keras Conv2D -- plus 2-D loads of the W_hi / W_lo [BN x 64] blocks.
+//                Everything lands in SWIZZLE_128B K-major layout (one pixel = one 128 B row).
+//   warps 0-7  : two consumer warpgroups, one per 64-pixel half of the tile.  Per K block 4 k-steps x 3 passes
+//                A_hi*W_hi + A_hi*W_lo + A_lo*W_hi (split-precision product, fp32 accumulators in registers),
+//                then the epilogue from the registers: + bias, LeakyReLU, re-split to hi/lo 16-bit planes, stores
+//                into the destination channel slice (which is how channel concats and the NN-upsample parity
+//                scatter are realised without extra passes).
 //
-// mbarrier pipeline: full[s] (TMA -> MMA, tx-count), empty[s] (MMA -> TMA, via tcgen05.commit),
-// tmem_full (MMA -> epilogue).  A watchdog turns a stuck barrier into a trap instead of a hang.
+// mbarrier pipeline: full[s] (TMA -> MMA, tx-count), empty[s] (MMA -> TMA, one arrive per warpgroup once its
+// wgmma reading the stage retired).  A watchdog turns a stuck barrier into a trap instead of a hang.
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <cstdio>
@@ -33,26 +30,24 @@ namespace film {
 namespace {
 using namespace tc;
 
-constexpr int kNumThreads = 192;
+constexpr int kConsumers = 256;                 // two warpgroups
+constexpr int kNumThreads = kConsumers + 128;   // + the producer warpgroup (one active warp)
 template <int BN, int KC>
 struct TcCfg {
   static constexpr int kABytes = kTileM * KC * 2;  // 16 KiB (KC = 64) or 8 KiB (KC = 32) per plane
   static constexpr int kWBytes = BN * KC * 2;
   static constexpr int kStageBytes = 2 * kABytes + 2 * kWBytes;
-  // Small-N tiles have short K loops and are bound by per-tile serialisation (prologue ->
-  // mainloop -> epilogue), not by pipeline depth: give them 2 stages and 2 CTAs per SM so one
-  // CTA's epilogue overlaps the other's mainloop (ncu, profiles/r1_ncu_conv.md).
   static constexpr int kStages = (BN == 256) ? 2 : (BN == 128) ? 3 : 2;
-  static constexpr int kMinBlocks = (BN <= 64) ? 2 : 1;
-  // fused-N product for BN <= 128 (see film_conv3x3_tc.cu): accumulator = 2*BN columns
+  // two-accumulator product for BN <= 128: A_hi x W_hi and A_lo x W_hi accumulate into the first BN columns,
+  // A_hi x W_lo into the second BN columns (all wgmma of one shape); the epilogue adds the halves
   static constexpr bool kFused = BN <= 128;
-  static constexpr int kTmemCols = kFused ? 2 * BN : BN;
-  // stages + barriers (8 B each) + tmem ptr + bias + flow-head weights
+  static constexpr int kAccRegs = (kFused ? 2 * BN : BN) / 2;
+  // stages + barriers (8 B each) + bias + flow-head weights
   static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 + BN * 4 + BN * 8 + 16;
 };
 
 template <int BN, int KC>
-__global__ void __launch_bounds__(kNumThreads, TcCfg<BN, KC>::kMinBlocks) k_conv_tc(const ConvProblem* __restrict__ prob_base) {
+__global__ void __launch_bounds__(kNumThreads, 1) k_conv_tc(const ConvProblem* __restrict__ prob_base) {
   using Cfg = TcCfg<BN, KC>;
   // grid.z selects one of `group` consecutive problems with identical grids (the four parity classes
   // of the NN-upsample + 2x2 conv are one launch)
@@ -65,12 +60,8 @@ __global__ void __launch_bounds__(kNumThreads, TcCfg<BN, KC>::kMinBlocks) k_conv
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* gen_base = smem_raw + (base - raw);
   const uint32_t bar_base = base + Cfg::kStages * Cfg::kStageBytes;
-  // barriers: full[kStages], empty[kStages], tmem_full ; then tmem ptr ; then bias
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (Cfg::kStages + s); };
-  const uint32_t tmem_full_bar = bar_base + 8u * (2 * Cfg::kStages);
-  uint32_t* tmem_ptr_smem =
-      reinterpret_cast<uint32_t*>(gen_base + Cfg::kStages * Cfg::kStageBytes + 8 * (2 * Cfg::kStages + 1));
   float* bias_smem = reinterpret_cast<float*>(gen_base + Cfg::kStages * Cfg::kStageBytes + 256);
   float* w4_smem = bias_smem + BN;  // [BN][2] + b4[2], flow-head mode only
 
@@ -94,28 +85,25 @@ __global__ void __launch_bounds__(kNumThreads, TcCfg<BN, KC>::kMinBlocks) k_conv
   int nkb = 0;
   for (int s = 0; s < nsrc; ++s) nkb += prob->src[s].nchunk * ntaps;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     for (int s = 0; s < Cfg::kStages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 2);   // one arrive per consumer warpgroup
     }
-    mbar_init(tmem_full_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(smem_u32(tmem_ptr_smem), (uint32_t)Cfg::kTmemCols);
-  if (warp >= 2) {
-    for (int i = threadIdx.x - 64; i < BN; i += 128) bias_smem[i] = (n0 + i < cout) ? prob->bias[n0 + i] : 0.f;
+  if (warp < 8) {
+    for (int i = threadIdx.x; i < BN; i += kConsumers) bias_smem[i] = (n0 + i < cout) ? prob->bias[n0 + i] : 0.f;
     if (epi_mode == 1) {
-      for (int i = threadIdx.x - 64; i < 2 * BN; i += 128) w4_smem[i] = (i < 2 * cout) ? prob->head_w4[i] : 0.f;
-      if (threadIdx.x - 64 < 2) w4_smem[2 * BN + threadIdx.x - 64] = prob->head_b4[threadIdx.x - 64];
+      for (int i = threadIdx.x; i < 2 * BN; i += kConsumers) w4_smem[i] = (i < 2 * cout) ? prob->head_w4[i] : 0.f;
+      if (threadIdx.x < 2) w4_smem[2 * BN + threadIdx.x] = prob->head_b4[threadIdx.x];
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
+  if (warp >= 8) {
+    regs_dec<40>();   // registers of the producer warpgroup go to the consumers (168 per thread at launch)
+    if (warp > 8) return;
     // ===================== TMA producer (warp-uniform, elected lane issues) =====================
     const CUtensorMap* tm_w_hi = &prob->tm_w_hi;
     const CUtensorMap* tm_w_lo = &prob->tm_w_lo;
@@ -146,81 +134,85 @@ __global__ void __launch_bounds__(kNumThreads, TcCfg<BN, KC>::kMinBlocks) k_conv
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (warp-uniform, elected lane issues) =====================
-    const uint32_t idesc = make_idesc<BN>();
-    const uint32_t idesc2 = make_idesc<(Cfg::kFused ? 2 * BN : BN)>();
-    for (int kb = 0; kb < nkb; ++kb) {
-      const int stage = kb % Cfg::kStages;
-      const uint32_t phase = (uint32_t)(kb / Cfg::kStages) & 1u;
-      mbar_wait(full_bar(stage), phase);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t sa = base + stage * Cfg::kStageBytes;
-        const uint64_t a_hi = make_desc_kc<KC>(sa), a_lo = make_desc_kc<KC>(sa + kABytes);
-        const uint64_t w_hi = make_desc_kc<KC>(sa + 2 * kABytes), w_lo = make_desc_kc<KC>(sa + 2 * kABytes + Cfg::kWBytes);
-        const uint32_t first = kb == 0 ? 0u : 1u;
+    return;
+  }
+
+  // ===================== consumer warpgroups: MMA + epilogue =====================
+  regs_inc<232>();
+  const int wg = warp >> 2;                  // which 64-pixel half of the tile
+  const uint32_t a_row0 = (uint32_t)(wg * 64 * KC * 2);
+  float acc[Cfg::kAccRegs];
 #pragma unroll
-        for (int k = 0; k < KC / 16; ++k) {
-          const uint64_t adv = (uint64_t)(k * 32 >> 4);  // 16 elements x 2 B = 32 B along K
-          if (one) {
-            umma(tmem_base, a_hi + adv, w_hi + adv, idesc, k == 0 ? first : 1u);
-          } else if constexpr (Cfg::kFused) {
-            umma(tmem_base, a_hi + adv, w_hi + adv, idesc2, k == 0 ? first : 1u);  // [W_hi ; W_lo]
-            umma(tmem_base, a_lo + adv, w_hi + adv, idesc, 1u);
-          } else {
-            umma(tmem_base, a_lo + adv, w_hi + adv, idesc, k == 0 ? first : 1u);
-            umma(tmem_base, a_hi + adv, w_lo + adv, idesc, 1u);
-            umma(tmem_base, a_hi + adv, w_hi + adv, idesc, 1u);
-          }
-        }
-        umma_commit(empty_bar(stage));
-        if (kb == nkb - 1) umma_commit(tmem_full_bar);
+  for (int i = 0; i < Cfg::kAccRegs; ++i) acc[i] = 0.f;
+  int prev_stage = -1;
+  for (int kb = 0; kb < nkb; ++kb) {
+    const int stage = kb % Cfg::kStages;
+    const uint32_t phase = (uint32_t)(kb / Cfg::kStages) & 1u;
+    mbar_wait(full_bar(stage), phase);
+    const uint32_t sa = base + stage * Cfg::kStageBytes;
+    const uint64_t a_hi = make_desc_kc<KC>(sa + a_row0), a_lo = make_desc_kc<KC>(sa + kABytes + a_row0);
+    const uint64_t w_hi = make_desc_kc<KC>(sa + 2 * kABytes), w_lo = make_desc_kc<KC>(sa + 2 * kABytes + Cfg::kWBytes);
+    const uint32_t first = kb == 0 ? 0u : 1u;
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < KC / 16; ++k) {
+      const uint64_t adv = (uint64_t)(k * 32 >> 4);  // 16 elements x 2 B = 32 B along K
+      if (one) {
+        wgmma<BN>(acc, a_hi + adv, w_hi + adv, k == 0 ? first : 1u);
+      } else if constexpr (Cfg::kFused) {
+        wgmma<BN>(acc, a_hi + adv, w_hi + adv, k == 0 ? first : 1u);
+        wgmma<BN>(acc + BN / 2, a_hi + adv, w_lo + adv, k == 0 ? first : 1u);
+        wgmma<BN>(acc, a_lo + adv, w_hi + adv, 1u);
+      } else {
+        wgmma<BN>(acc, a_lo + adv, w_hi + adv, k == 0 ? first : 1u);
+        wgmma<BN>(acc, a_hi + adv, w_lo + adv, 1u);
+        wgmma<BN>(acc, a_hi + adv, w_hi + adv, 1u);
       }
-      __syncwarp();
     }
-  } else {
-    // ===================== epilogue (warps 2..5) =====================
-    const int q = warp & 3;                 // TMEM lane quarter this warp may access
-    const int r = q * 32 + lane;            // tile row == TMEM lane
+    wgmma_commit();
+    // the previous K block's wgmma group has retired once at most this one is in flight: release its stage
+    wgmma_wait<1>();
+    if (prev_stage >= 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty_bar(prev_stage));
+    prev_stage = stage;
+  }
+  wgmma_wait<0>();
+  acc_fence<Cfg::kAccRegs>(acc);
+
+  // fragment -> pixels: this thread holds rows r0 = 64 wg + 16 (warp & 3) + lane / 4 and r0 + 8, channel pairs
+  // 8j + 2 (lane & 3) + {0, 1}
+  const bool fused3 = Cfg::kFused && !one;
+  auto value = [&](int h, int j, int e) {
+    const int i = 4 * j + 2 * h + e;
+    return fused3 ? acc[i] + acc[(i + BN / 2) % Cfg::kAccRegs] : acc[i];
+  };
+  const int q = lane & 3;
+  const float* head_vup = prob->head_vup;
+  float* head_res = prob->head_res;
+  float* head_v = prob->head_v;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
     const int py = y0 + r / tile_w, px = x0 + r % tile_w;
     const bool valid = (py < prob->H) && (px < prob->W);
     const int64_t opix = ((int64_t)b * prob->out_H + ((int64_t)py * prob->out_sy + prob->out_oy)) * prob->out_W +
                          ((int64_t)px * prob->out_sx + prob->out_ox);
-    const int act = prob->act;
-    sp_t* oh = prob->out_hi + opix * prob->out_C + prob->out_c_off + n0;
-    sp_t* ol = prob->out_lo + opix * prob->out_C + prob->out_c_off + n0;
-    const bool lo_skip = prob->out_lo_skip != 0;
-    const float* head_vup = prob->head_vup;
-    float* head_res = prob->head_res;
-    float* head_v = prob->head_v;
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    const uint32_t t_addr = tmem_base + ((uint32_t)(q * 32) << 16);
     if (epi_mode == 1) {
       // flow head: hidden = LeakyReLU(acc + b3) stays in fp32 registers; 2-wide linear layer + v_up
       float r0 = 0.f, r1 = 0.f;
-#pragma unroll 1
-      for (int cc = 0; cc < BN / 32; ++cc) {
-        uint32_t v[32];
-        tmem_ld32(t_addr + (uint32_t)(cc * 32), v);
-        if (Cfg::kFused && !one) {
-          uint32_t u[32];
-          tmem_ld32(t_addr + (uint32_t)(BN + cc * 32), u);
-          tmem_ld_wait();
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(u[j]));
-        } else {
-          tmem_ld_wait();
-        }
+      for (int j = 0; j < BN / 8; ++j)
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float hdn = leaky(__uint_as_float(v[j]) + bias_smem[cc * 32 + j]);
-          r0 = fmaf(hdn, w4_smem[(cc * 32 + j) * 2], r0);
-          r1 = fmaf(hdn, w4_smem[(cc * 32 + j) * 2 + 1], r1);
+        for (int e = 0; e < 2; ++e) {
+          const int c = 8 * j + 2 * q + e;
+          const float hdn = leaky(value(h, j, e) + bias_smem[c]);
+          r0 = fmaf(hdn, w4_smem[c * 2], r0);
+          r1 = fmaf(hdn, w4_smem[c * 2 + 1], r1);
         }
-      }
-      if (valid) {
+      r0 += __shfl_xor_sync(0xffffffffu, r0, 1);
+      r1 += __shfl_xor_sync(0xffffffffu, r1, 1);
+      r0 += __shfl_xor_sync(0xffffffffu, r0, 2);
+      r1 += __shfl_xor_sync(0xffffffffu, r1, 2);
+      if (valid && q == 0) {
         float2 res = make_float2(r0 + w4_smem[2 * BN], r1 + w4_smem[2 * BN + 1]);
         float2 tot = res;
         if (head_vup) {
@@ -231,42 +223,30 @@ __global__ void __launch_bounds__(kNumThreads, TcCfg<BN, KC>::kMinBlocks) k_conv
         reinterpret_cast<float2*>(head_res)[opix] = res;
         reinterpret_cast<float2*>(head_v)[opix] = tot;
       }
-    } else {
-#pragma unroll 1
-      for (int cc = 0; cc < BN / 32; ++cc) {
-        if (n0 + cc * 32 >= cout) break;
-        uint32_t v[32];
-        tmem_ld32(t_addr + (uint32_t)(cc * 32), v);
-        if (Cfg::kFused && !one) {
-          uint32_t u[32];
-          tmem_ld32(t_addr + (uint32_t)(BN + cc * 32), u);
-          tmem_ld_wait();
+    } else if (valid) {
+      const int act = prob->act;
+      sp_t* oh = prob->out_hi + opix * prob->out_C + prob->out_c_off + n0;
+      sp_t* ol = prob->out_lo + opix * prob->out_C + prob->out_c_off + n0;
+      const bool lo_skip = prob->out_lo_skip != 0;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(v[j]) + __uint_as_float(u[j]));
-        } else {
-          tmem_ld_wait();
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + 2 * q;
+        if (n0 + c >= cout) break;
+        float f0 = value(h, j, 0) + bias_smem[c], f1 = value(h, j, 1) + bias_smem[c + 1];
+        if (act) {
+          f0 = leaky(f0);
+          f1 = leaky(f1);
         }
-        if (valid) {
-#pragma unroll
-          for (int g = 0; g < 2; ++g) {
-            float f[16];
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              float x = __uint_as_float(v[g * 16 + j]) + bias_smem[cc * 32 + g * 16 + j];
-              f[j] = act ? leaky(x) : x;
-            }
-            if (lo_skip) pack_store16_hi(f, oh + cc * 32 + g * 16);
-            else pack_store16(f, oh + cc * 32 + g * 16, ol + cc * 32 + g * 16);
-          }
+        uint32_t hi, lo;
+        if (lo_skip) {
+          *reinterpret_cast<uint32_t*>(oh + c) = pack2_hi(f0, f1);
+        } else {
+          split_pack2(f0, f1, hi, lo);
+          *reinterpret_cast<uint32_t*>(oh + c) = hi;
+          *reinterpret_cast<uint32_t*>(ol + c) = lo;
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)Cfg::kTmemCols);
   }
 }
 

@@ -1,4 +1,4 @@
-// Host side of the FILM B200 engine: weight loading + repacking, per-shape execution plans
+// Host side of the FILM engine: weight loading + repacking, per-shape execution plans
 // (arena, TMA tensor maps, static kernel schedule captured in a CUDA graph) and the C ABI of
 // include/film_b200.h.  Network wiring follows the reference graph,
 // models/film_net/interpolator.py:120-207; each step cites the lines it replaces.
@@ -47,8 +47,7 @@ struct Error {
 // Precision plan.  Every tensor-core conv call site belongs to a STAGE; bit s of the plan's one-pass mask
 // selects the single-pass product (A_hi x W_hi: fp16 operands, fp32 accumulate) for stage s, otherwise the
 // three-pass split product (fp32-grade).  The flow heads and the RGB head are always three-pass / fp32.
-// The default mask is the outcome of the measured per-stage error study (tools/precision_study.py,
-// profiles/r2_precision_study_1080p.md, DESIGN.md section 3).
+// The default mask is the outcome of a measured per-stage error study (tools/precision_study.py).
 // ----------------------------------------------------------------------------------------
 enum Stage {
   ST_FE_I0_K01 = 0, ST_FE_I0_K23, ST_FE_I0_K45, ST_FE_I0_K67,  // sub-tree of image level 0: conv pairs
@@ -462,12 +461,11 @@ struct DebugTensor {
 struct Plan {
   int h, w, H, W, off_y, off_x;
   int conv_impl;
-  int conv3x3_v2 = 1, num_sms = 148, conv3x3_2cta = 0;
-  int conv3x3_halo = 0;  // 1: pair kernel, 2: + single-CTA persistent kernel, 3: + 32-channel-chunk layers
+  int conv3x3_v2 = 1, num_sms = 132, conv3x3_2cta = 0;
+  int conv3x3_halo = 0;  // 1: CTA-pair layers, 2: + every persistent layer (64-channel chunks), 3: + 32-channel chunks
   uint32_t onepass_mask = 0;  // precision plan: stages on the single-pass product
   int fe_conv0_tc = 0;        // 1: cfeat_conv_0 on the tensor cores (32-channel-padded image), 0: fp32 FMA kernel
   int fuse_rgb_head = 1;      // RGB head + crop in the epilogue of the decoder's last conv
-  int conv3x3_dual = 0;       // CTA-pair kernel: two spatial items per streamed weight pass
   int fuse_flow_head = 1;     // flow head (conv_3, conv_4, residual add) in conv_2 epilogue: 1 = level 0, 2 = levels 0 and 1
   int plane_skip = 1;         // lo planes that no consumer reads are neither gathered nor written
   int mma_straight = 1;       // straight-line MMA issue for resident weights
@@ -477,7 +475,7 @@ struct Plan {
   ConvProblem* d_probs = nullptr;
   struct Op {
     std::function<cudaError_t(cudaStream_t)> fn;
-    int category;      // 0 = tcgen05 conv, 1 = warp gather, 2 = other bandwidth kernels
+    int category;      // 0 = tensor-core conv, 1 = warp gather, 2 = other bandwidth kernels
     std::string name;
     double flops;      // reference-graph FLOPs (convs) of this op
     double bytes;      // algorithmic bytes (gathers)
@@ -602,16 +600,12 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
                   (kc == kChunk || pc.cout <= 64);
   cp.epi_mode = epi_mode;
   int box_h, box_w;
-  // CTA-pair kernel: large levels only (it needs 16x8 tiles and enough tile pairs to fill the SM pairs)
-  const bool want_pair = v2 && P.conv3x3_2cta && epi_mode < 2 &&   // (the RGB / flow-head epilogues live in the single-CTA kernel)
-                         (P.conv3x3_2cta >= 2 ||  // >= 2: every eligible layer (testing)
-                          (long)cp.B * ((cp.H + 15) / 16) * ((cp.W + 7) / 8) >= 4L * P.num_sms);
   if (v2) {
-    if (pool_out || want_pair) {
-      cp.tile_h = 16;  // the fused pool maps 2x2 partners to lanes l^1 / l^8 of a 16x8 tile
+    if (pool_out) {
+      cp.tile_h = 16;  // the fused pool of a 16x8 tile finds each 2x2 partner in lane ^ 4 and the thread's second fragment row
       cp.tile_w = 8;
     } else {
-      conv3x3_tc_pick_tile(cp.H, cp.W, cp.B, pc.cout, P.num_sms, cp.tile_h, cp.tile_w);
+      conv3x3_tc_pick_tile(cp.H, cp.W, cp.B, pc.cout, kc, cp.passes, pc.ktot, epi_mode, P.num_sms, cp.tile_h, cp.tile_w);
     }
     box_h = cp.tile_h + 2;
     box_w = cp.tile_w;
@@ -683,26 +677,20 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
     cp.pool_C = pool_out->C;
   }
   cp.group = 1;
-  cp.pair = 0;
-  bool pair = false;
-  // wide halo level: 1 = pair kernel, 2 = + single-CTA kernel (64-channel chunks), 3 = + 32-channel chunks
-  // (SWIZZLE_64B descriptor offsets verified by tools/ubench/desc_offset_test.cu; kernels not yet timed)
+  // wide halo level: 1 = CTA-pair layers, 2 = + every persistent layer (64-channel chunks), 3 = + 32-channel chunks
   int halo_ok = (v2 && cp.tile_h == 16 && cp.tile_w == 8) ? P.conv3x3_halo : 0;
   if (kc != kChunk && halo_ok < 3) halo_ok = 0;
   cp.halo = halo_ok >= 2;
-  if (v2) conv3x3_tc_plan(cp, P.num_sms);
-  // the pair kernel pays off where weights are re-streamed per tile (halved weight bytes per CTA);
-  // layers whose weights stay resident in one CTA's smem are faster on the single-CTA fused kernel
-  // (measured at 1080p, profiles/r1k: resident 9-K-block layers lose ~15 % on the pair kernel, the
-  // 18-K-block 128->32 flow conv gains 28 %)
-  if (want_pair && (!cp.v2_resident || cp.ktot / cp.kchunk >= 18 || P.conv3x3_2cta >= 2)) {
-    ConvProblem alt = cp;
-    alt.halo = halo_ok >= 1;
-    alt.dual = P.conv3x3_dual;
-    if (conv3x3_tc2_plan(alt, P.num_sms)) {
-      cp = alt;
-      pair = true;
-    }
+  if (v2 && !conv3x3_tc_plan(cp, P.num_sms))
+    throw Error{FILM_ERR_UNSUPPORTED, "persistent 3x3 conv: shared-memory rings do not fit (" + tag + ")"};
+  // CTA pair ((2,1,1) clusters sharing every streamed weight tap by TMA multicast): layers that stream their weights, on the
+  // large levels (conv3x3_2cta = 1) or on every level (2); the RGB / flow-head epilogues stay on single CTAs
+  if (v2 && P.conv3x3_2cta && epi_mode < 2 && !cp.v2_resident &&
+      (P.conv3x3_2cta >= 2 || (long)cp.B * cp.tiles_y * cp.tiles_x >= 4L * P.num_sms)) {
+    cp.pair = 1;
+    if (halo_ok >= 1) cp.halo = 1;
+    if (!conv3x3_tc_plan(cp, P.num_sms))
+      throw Error{FILM_ERR_UNSUPPORTED, "persistent 3x3 conv: shared-memory rings do not fit (" + tag + ")"};
   }
   if (cp.halo) {  // the chosen kernel loads (tile_w + 2)-pixel-wide halo boxes
     for (int s = 0; s < cp.nsrc; ++s) {
@@ -716,7 +704,7 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   // issued tensor-core work: 3 passes over the padded K and the padded tile grid
   double k_issued = 0;  // skipped all-zero k-steps are not issued work
   for (size_t si = 0; si < pc.src_chunks.size(); ++si)
-    k_issued += (double)pc.src_chunks[si] * pc.ntaps * ((v2 || pair) ? pc.src_ksteps[si] * 16 : pc.kchunk);
+    k_issued += (double)pc.src_chunks[si] * pc.ntaps * (v2 ? pc.src_ksteps[si] * 16 : pc.kchunk);
   P.mma_flops += (double)cp.passes * 2.0 * (double)cp.B * cp.tiles_y * cp.tiles_x * kTileM * k_issued *
                  (double)(((pc.cout + bn - 1) / bn) * bn);
   // algorithmic HBM bytes of this call site: every source plane it consumes read once, every destination plane written once
@@ -734,9 +722,8 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   if (no_op) return idx;  // the caller launches this problem as part of a group
   Plan* pp = &P;
   const int impl = P.conv_impl;
-  P.add_op(0, tag, [pp, idx, impl, v2, pair](cudaStream_t st) {
+  P.add_op(0, tag, [pp, idx, impl, v2](cudaStream_t st) {
     if (impl == 1) return launch_conv_simt(pp->d_probs + idx, pp->h_probs[idx], st);
-    if (pair) return launch_conv3x3_tc2(pp->d_probs + idx, pp->h_probs[idx], st);
     return v2 ? launch_conv3x3_tc(pp->d_probs + idx, pp->h_probs[idx], st)
               : launch_conv_tc(pp->d_probs + idx, pp->h_probs[idx], st);
   }, 2.0 * ref_macs_per_px * (double)cp.B * cp.H * cp.W, alg_bytes);
@@ -750,7 +737,6 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
   Plan& P = *pl;
   P.fe_conv0_tc = fe_conv0_tc & 1;
   P.fuse_rgb_head = (fe_conv0_tc & 2) ? 0 : 1;
-  P.conv3x3_dual = (fe_conv0_tc & 4) ? 1 : 0;
   P.plane_skip = (fe_conv0_tc & 8) ? 0 : 1;
   P.fuse_flow_head = (fe_conv0_tc & 64) ? 0 : ((fe_conv0_tc & 128) ? 2 : 1);
   P.mma_straight = (fe_conv0_tc & 16) ? 0 : 1;
@@ -958,14 +944,14 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
     add_conv(P, "flow_conv0" + lt, 9.0 * 2 * C * nf, M.flow[p][0], flow_src, 1, c0, 0, ST_FLOW_L0 + l, ST_FLOW_L0 + l);
     add_conv(P, "flow_conv1" + lt, 9.0 * nf * nf, M.flow[p][1], {{c0, 0}}, 1, c1, 0, ST_FLOW_L0 + l, ST_FLOW_L0 + l);
     // level 0 (32-filter predictor): conv_3, conv_4 and the residual add run in conv_2's epilogue.  The kernel supports
-    // nf <= 64, but per-op timing (profiles/r2e) shows the 64-filter level 1 epilogue-bound (32 x 32 FMAs per thread):
-    // 0.253 ms fused vs 0.224 ms as two launches, while level 0 gains (0.502 vs 0.566 ms) -- so only level 0 is fused.
+    // nf <= 64, but the 64-filter level 1 epilogue (32 x 32 FMAs per pixel) is slower fused than as two launches
+    // while level 0 gains -- so by default only level 0 is fused (fuse_flow_head = 2 fuses both).
     const bool fuse_head = P.conv_impl == 0 && P.conv3x3_v2 && P.fuse_flow_head && nf <= (P.fuse_flow_head >= 2 ? 64 : 32);
     if (fuse_head) {
       const size_t ci = add_conv(P, "flow_conv2+head" + lt, 9.0 * nf * nf + 1.0 * nf * (nf / 2) + (nf / 2) * 2.0, M.flow[p][2],
                                  {{c1, 0}}, 1, nullptr, 0, ST_FLOW_L0 + l, ST_NONE, 1, 1, 0, 0, nullptr, false, 3);
       ConvProblem& hp = P.h_probs[ci];
-      if (hp.bn != nf || hp.pair) throw Error{FILM_ERR_UNSUPPORTED, "flow-head epilogue expects one N tile on the single-CTA kernel"};
+      if (hp.bn != nf) throw Error{FILM_ERR_UNSUPPORTED, "flow-head epilogue expects one N tile on the single-CTA kernel"};
       hp.head_w3 = M.flow_w3[p];
       hp.head_b3 = M.flow_b3[p];
       hp.head_w4 = M.flow_w4[p];
@@ -1131,7 +1117,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
     P.signal_last(P.tok_end);
   }
 
-  // reference-graph conv FLOPs (frame_interpolation_b200/spec.py conv_macs, SURVEY.md 8d)
+  // reference-graph conv FLOPs (frame_interpolation_b200/spec.py conv_macs)
   {
     double fe = 0, fl = 0, fu = 0;
     for (int i = 0; i < kLevels; ++i) {
@@ -1199,23 +1185,20 @@ struct film_handle {
   cudaEvent_t fork_event = nullptr;
   int use_lanes = 0;   // stream lanes measured no gain at 1080p (smem-saturating kernels cannot co-reside)
   int conv3x3_v2 = 1;  // persistent tap-reuse kernel for 3x3 convs
-  int conv3x3_2cta = 1;  // CTA-pair (cta_group::2) kernel for streamed-weight 3x3 convs on the large levels
-  int conv3x3_halo = 3;  // wide halo boxes (one 10-px box per chunk serves nine taps): 0 off, 1 pair kernel, 2 both
-                         // persistent kernels, 3 also the 32-channel-chunk layers (default: validated on hardware in
-                         // round 2, -0.6 % / -2.0 % step time in two same-box A/Bs, profiles/r2c|r2d_variants_ab.md)
+  int conv3x3_2cta = 0;  // CTA-pair clusters for the streamed-weight 3x3 convs of the large levels: off by default, 1080p
+                         // step 60.5 ms with them against 53.4 ms without (H100 SXM, 400 W; the paired layers run slower)
+  int conv3x3_halo = 3;  // wide halo boxes (one 10-px box per chunk serves nine taps): 0 off, 1 the CTA-pair layers, 2 every
+                         // 64-channel-chunk layer of the persistent kernel, 3 also its 32-channel-chunk layers
   uint32_t onepass_mask = kDefaultOnepassMask;  // precision plan (see `enum Stage`)
   int fe_conv0_tc = 0;  // cfeat_conv_0: 0 = register-tiled fp32 FMA kernel straight from the fp32 image (default: exact fp32,
                         // no widened image tensor; K = 27 is not tensor-core work), 1 = tensor-core kernel over the
-                        // 32-channel-padded image (per-op timing of profiles/r2e: 0.78 ms over the 7 levels against 0.87 ms,
-                        // i.e. 0.6 % of the step -- inside the run-to-run noise of the whole-step A/B)
+                        // 32-channel-padded image
   int fuse_rgb_head = 1;  // 1 = RGB head + crop in the epilogue of fusion_conv2@L0 (default), 0 = separate kernel
-  int conv3x3_dual = 1;   // 1 = CTA-pair kernel serves two spatial items per streamed weight pass (default: -2.3 % step
-                          // time in the same-box A/B of profiles/r2d_variants_ab.md)
-  int plane_skip = 1, mma_straight = 1, arena_reuse = 1;   // round-2 optimisations, individually switchable (A/B, bisecting)
+  int plane_skip = 1, mma_straight = 1, arena_reuse = 1;   // optimisations, individually switchable (A/B, bisecting)
   int fuse_flow_head = 1;
   uint8_t* u8_stage = nullptr;  // film_interpolate_u8: [x0][x1][out] on the device
   size_t u8_bytes = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   std::vector<cudaEvent_t> op_events;
   film_profile_t prof;
 };
@@ -1282,14 +1265,14 @@ static void drop_plans(film_handle* h) {
 static Plan* get_plan(film_handle* h, int hh, int ww, int align) {
   char key[96];
   snprintf(key, sizeof(key), "%dx%d_a%d_i%d_v%d_l%d_p%d_h%d_m%x_d%d", hh, ww, align > 0 ? align : 0, h->conv_impl, h->conv3x3_v2,
-           h->use_lanes, h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->keep_debug * 256 + h->fuse_flow_head * 64 + h->arena_reuse * 32 + h->mma_straight * 16 + h->plane_skip * 8 + h->conv3x3_dual * 4 +
+           h->use_lanes, h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->keep_debug * 256 + h->fuse_flow_head * 64 + h->arena_reuse * 32 + h->mma_straight * 16 + h->plane_skip * 8 +
                h->fuse_rgb_head * 2 + h->fe_conv0_tc);
   auto it = h->plans.find(key);
   if (it != h->plans.end()) return it->second.get();
   std::unique_ptr<Plan> p;
   try {
     p = build_plan(*h->model, hh, ww, align, h->conv_impl, h->keep_debug != 0, h->conv3x3_v2, h->num_sms,
-                   h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->use_lanes != 0, h->fe_conv0_tc | (h->fuse_rgb_head ? 0 : 2) | (h->conv3x3_dual ? 4 : 0) | (h->plane_skip ? 0 : 8) |
+                   h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->use_lanes != 0, h->fe_conv0_tc | (h->fuse_rgb_head ? 0 : 2) | (h->plane_skip ? 0 : 8) |
                        (h->mma_straight ? 0 : 16) | (h->arena_reuse ? 0 : 32) | (h->fuse_flow_head ? 0 : 64) |
                        (h->fuse_flow_head >= 2 ? 128 : 0));
   } catch (const Error& e0) {
@@ -1299,7 +1282,7 @@ static Plan* get_plan(film_handle* h, int hh, int ww, int align) {
     if (h->plans.empty()) throw;
     drop_plans(h);
     p = build_plan(*h->model, hh, ww, align, h->conv_impl, h->keep_debug != 0, h->conv3x3_v2, h->num_sms,
-                   h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->use_lanes != 0, h->fe_conv0_tc | (h->fuse_rgb_head ? 0 : 2) | (h->conv3x3_dual ? 4 : 0) | (h->plane_skip ? 0 : 8) |
+                   h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->use_lanes != 0, h->fe_conv0_tc | (h->fuse_rgb_head ? 0 : 2) | (h->plane_skip ? 0 : 8) |
                        (h->mma_straight ? 0 : 16) | (h->arena_reuse ? 0 : 32) | (h->fuse_flow_head ? 0 : 64) |
                        (h->fuse_flow_head >= 2 ? 128 : 0));
   }
@@ -1354,8 +1337,8 @@ static void run_plan(film_handle* h, Plan* P, cudaStream_t st) {
 extern "C" {
 
 const char* film_version(void) {
-  return "film_b200 0.2 sm_100a split=" FILM_SPLIT_NAME
-         " mma=tcgen05.kind::f16, per-stage precision plan: 3-pass (hi*hi+hi*lo+lo*hi) or 1-pass (hi*hi)";
+  return "film_b200 0.3 sm_90a split=" FILM_SPLIT_NAME
+         " mma=wgmma.f32, per-stage precision plan: 3-pass (hi*hi+hi*lo+lo*hi) or 1-pass (hi*hi)";
 }
 
 int film_create(film_handle** out, const char* weights_path, int device_ordinal) {
@@ -1368,14 +1351,14 @@ int film_create(film_handle** out, const char* weights_path, int device_ordinal)
   try {
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
-      throw Error{FILM_ERR_CUDA, "no CUDA device: the FILM B200 engine has no CPU fallback"};
+      throw Error{FILM_ERR_CUDA, "no CUDA device: the FILM engine has no CPU fallback"};
     if (device_ordinal < 0 || device_ordinal >= ndev) throw Error{FILM_ERR_ARG, "bad device ordinal"};
     FILM_CUDA(cudaSetDevice(device_ordinal));
     cudaDeviceProp prop;
     FILM_CUDA(cudaGetDeviceProperties(&prop, device_ordinal));
-    if (prop.major != 10)
+    if (prop.major != 9 || prop.minor != 0)
       throw Error{FILM_ERR_CUDA, std::string("device is sm_") + std::to_string(prop.major * 10 + prop.minor) +
-                                     ", this engine is sm_100a-only (tcgen05/TMEM/TMA)"};
+                                     ", this engine is sm_90a-only (wgmma/TMA)"};
     h = new film_handle;
     h->device = device_ordinal;
     memset(&h->prof, 0, sizeof(h->prof));
@@ -1383,12 +1366,10 @@ int film_create(film_handle** out, const char* weights_path, int device_ordinal)
     for (auto& e : h->ev) FILM_CUDA(cudaEventCreate(&e));
     FILM_CUDA(conv_tc_configure());
     FILM_CUDA(conv3x3_tc_configure());
-    FILM_CUDA(conv3x3_tc2_configure());
     if (const char* e2 = getenv("FILM_2CTA")) h->conv3x3_2cta = atoi(e2);
     if (const char* e3 = getenv("FILM_HALO")) h->conv3x3_halo = atoi(e3);
     if (const char* e5 = getenv("FILM_FE0_TC")) h->fe_conv0_tc = atoi(e5) ? 1 : 0;
     if (const char* e6 = getenv("FILM_RGB_FUSE")) h->fuse_rgb_head = atoi(e6) ? 1 : 0;
-    if (const char* e7 = getenv("FILM_DUAL")) h->conv3x3_dual = atoi(e7) ? 1 : 0;
     if (const char* e8 = getenv("FILM_PLANE_SKIP")) h->plane_skip = atoi(e8) ? 1 : 0;
     if (const char* e11 = getenv("FILM_FLOW_HEAD_FUSE")) h->fuse_flow_head = atoi(e11) < 0 ? 0 : (atoi(e11) > 2 ? 2 : atoi(e11));
     if (const char* e9 = getenv("FILM_STRAIGHT")) h->mma_straight = atoi(e9) ? 1 : 0;
@@ -1458,7 +1439,6 @@ int film_set_option(film_handle* h, const char* name, int value) {
   else if (n == "onepass_default") h->onepass_mask = kDefaultOnepassMask;
   else if (n == "fe_conv0_tc") h->fe_conv0_tc = value ? 1 : 0;
   else if (n == "fuse_rgb_head") h->fuse_rgb_head = value ? 1 : 0;
-  else if (n == "conv3x3_dual") h->conv3x3_dual = value ? 1 : 0;
   else if (n == "plane_skip") h->plane_skip = value ? 1 : 0;
   else if (n == "fuse_flow_head") h->fuse_flow_head = value < 0 ? 0 : (value > 2 ? 2 : value);
   else if (n == "mma_straight") h->mma_straight = value ? 1 : 0;

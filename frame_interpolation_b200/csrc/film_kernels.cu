@@ -1,4 +1,4 @@
-// Bandwidth-bound kernels of the FILM engine (sm_100a): pooling, first conv (K = 27),
+// Bandwidth-bound kernels of the FILM engine (sm_90a): pooling, first conv (K = 27),
 // flow-upsample + warp gathers, flow / RGB heads, and the CUDA-core validation conv.
 // All activations are NHWC; feature tensors are in the split 2 x 16-bit format
 // (film_common.cuh).  Every kernel reads/writes 128-bit channel vectors.
@@ -396,7 +396,7 @@ cudaError_t launch_act_pool(const sp_t* in_hi, const sp_t* in_lo, int in_C, int 
 // Shared gather helpers.
 // TF2 bilinear resize (half-pixel centres):  src = (dst + 0.5) * in/out - 0.5
 // TFA dense_image_warp / interpolate_bilinear border rule: floor clamped to [0, size-2],
-// alpha clamped to [0, 1]  (SURVEY.md section 8c rules 4 and 6).
+// alpha clamped to [0, 1].
 // ------------------------------------------------------------------------------------------
 struct ResizeTap {
   int lo, hi;

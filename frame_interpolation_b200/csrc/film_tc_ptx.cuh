@@ -1,10 +1,9 @@
-// Inline-PTX wrappers for the sm_100a tensor-core path: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / fences) and the UMMA shared-memory + instruction descriptors.
-// Bit layouts follow cute::UMMA::SmemDescriptor / InstrDescriptor (CUTLASS mma_sm100_desc.hpp).
+// Inline-PTX wrappers for the sm_90a tensor-core path: mbarrier, TMA (cp.async.bulk.tensor) and warpgroup MMA
+// (wgmma.mma_async with both operands in shared memory, fp32 accumulators in registers).
+// Descriptor bit layout: PTX ISA "Matrix Descriptor Format" of wgmma (cute::GMMA::GmmaDescriptor).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
-#include <cstdio>
 #include <stdint.h>
 
 #include "film_conv.h"
@@ -34,17 +33,17 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug must surface as a launch failure, never as a hung GPU.
+// Bounded wait: a protocol bug must surface as a launch failure, never as a hung GPU.  No printf here: a function call
+// between wgmma.commit_group and wgmma.wait_group makes ptxas serialise every wgmma of the kernel (C7510).
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   if (mbar_try_wait(bar, parity)) return;
   const long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > 4000000000LL) {  // ~2 s at 2 GHz
-      printf("film conv_tc: mbarrier timeout (block %d,%d thread %d)\n", blockIdx.x, blockIdx.y,
-             threadIdx.x);
-      __trap();
-    }
+    if (clock64() - t0 > 4000000000LL) __trap();  // ~2 s at 2 GHz
   }
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0,
@@ -63,180 +62,16 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* tm,
       ::"r"(dst), "l"(tm), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor layout):
-// start>>4 [0,14), LBO>>4 [16,30) (unused for swizzled K-major, 1), SBO>>4 [32,46) = 1024 B
-// (8 rows x 128 B), version=1 [46,48), layout_type=SWIZZLE_128B(2) [61,64).
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
-// Same for a K chunk of KC channels per row: KC = 64 -> 128-byte rows, SWIZZLE_128B (type 2),
-// 8-row atom = 1024 B; KC = 32 -> 64-byte rows, SWIZZLE_64B (type 4), 8-row atom = 512 B.
-template <int KC>
-__device__ __forceinline__ uint64_t make_desc_kc(uint32_t saddr) {
-  constexpr uint64_t kType = (KC == 64) ? 2 : 4;
-  constexpr uint64_t kSbo = (KC == 64) ? 1024 : 512;
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(kSbo >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= kType << 61;
-  return d;
-}
-
-// Position in an mbarrier ring whose depth is a RUNTIME value: stage index + phase bit, advanced by
-// compare-and-wrap.  (`i % depth`, `(i / depth) & 1` compile to a ~25-instruction I2F / MUFU.RCP / F2I
-// sequence per use -- measurable in the per-tap issue path of the producer and MMA warps.)
-struct RingPos {
-  int stage = 0;
-  uint32_t phase = 0;
-  __device__ __forceinline__ void advance(int depth) {
-    if (++stage == depth) {
-      stage = 0;
-      phase ^= 1u;
-    }
-  }
-};
-
-// Division by a kernel-invariant divisor without the ~25-instruction I2F / MUFU.RCP / IABS sequence of a runtime `/`:
-// q = (x * ceil(2^40 / d)) >> 40 is exact whenever x * d < 2^40 (tile indices and tile counts are < 2^20 for every frame
-// this engine accepts); otherwise the plain division is used.  The per-tile decode tile -> (b, y0, x0) runs in every
-// producer and epilogue warp for every tile (source-level ncu, profiles/r2i_stalls_flow_L0.md).
-struct FastDiv {
-  uint64_t mul;
-  uint32_t d;
-  bool fast;
-  __device__ __forceinline__ FastDiv(int divisor, int max_x) : d((uint32_t)divisor) {
-    fast = (uint64_t)(uint32_t)max_x * d < (1ull << 40);
-    mul = ((1ull << 40) + d - 1) / d;
-  }
-  __device__ __forceinline__ void divmod(int x, int& q, int& r) const {
-    const uint32_t qq = fast ? (uint32_t)(((uint64_t)(uint32_t)x * mul) >> 40) : (uint32_t)x / d;
-    q = (int)qq;
-    r = x - (int)(qq * d);
-  }
-};
-
-// K-major swizzled descriptor with an explicit stride between 8-row groups.  The hardware applies the
-// swizzle XOR on ABSOLUTE smem address bits (7..9 -> 4..6; 7..8 -> 4..5 for SWIZZLE_64B) and base_offset stays
-// 0: measured on B200 with tools/ubench/desc_offset_test.cu -- the start address may sit at any row inside
-// the swizzle atom and SBO need not be a multiple of the atom (rows of a 10-pixel-wide halo box: SBO = 10 rows).
-template <int KC>
-__device__ __forceinline__ uint64_t make_desc_sbo(uint32_t saddr, uint32_t sbo_bytes) {
-  constexpr uint64_t kType = (KC == 64) ? 2 : 4;   // SWIZZLE_128B (128-byte rows) / SWIZZLE_64B (64-byte rows)
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(sbo_bytes >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= kType << 61;
-  return d;
-}
-
-// Instruction descriptor for kind::f16 (cute::UMMA::InstrDescriptor): c_format=F32 [4,6),
-// a_format [7,10), b_format [10,13) (0 = F16, 1 = BF16), K-major A and B, N>>3 [17,23), M>>4 [24,29).
-template <int BN>
-__device__ __forceinline__ uint32_t make_idesc() {  // BN = MMA N extent
-#ifdef FILM_SPLIT_FP16
-  constexpr uint32_t fmt = 0;
-#else
-  constexpr uint32_t fmt = 1;
-#endif
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(BN >> 3) << 17) |
-         ((uint32_t)(kTileM >> 4) << 24);
-}
-
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                     uint32_t accumulate) {
+// Multicast form: the box lands at the same smem offset in every CTA of `mask` and signals the barrier at the same
+// offset in each of them.
+__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1,
+                                               uint16_t mask) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(dst), "l"(tm), "r"(bar), "r"(c0), "r"(c1), "h"(mask)
       : "memory");
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-        "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-
-// L2 prefetch of a 4-D tile (no smem destination, no barrier): hides DRAM latency for data that a
-// later cp.async.bulk.tensor of the same box will fetch.
-__device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* tm, int c0, int c1, int c2, int c3) {
-  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];" ::"l"(tm), "r"(c0),
-               "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-// Warp-uniform leader election.  Role loops are executed by all 32 lanes (converged) and only the
-// elected lane issues TMA / tcgen05 instructions: with `if (lane == 0)` around a whole role the
-// compiler wraps every uniform-datapath instruction (UTCHMMA, UTMALDG) in ELECT/BRA.U.ANY
-// divergence loops and the single issuing thread becomes the bottleneck (ncu, profiles/).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------
-// CTA-pair (cta_group::2) forms: two CTAs of a cluster cooperate on one M = 256 MMA.  Each CTA
-// holds its own 128 rows of A and HALF of the B rows; the leader (cluster rank 0) issues the MMA
-// and owns the "full" barriers; commits are multicast to the same barrier offset in both CTAs.
-// PTX forms as in CUTLASS (SM100_TMA_2SM_LOAD_*, SM100_MMA_F16BF16_2x1SM_SS, umma_arrive_multicast_2x1SM).
-// ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -252,64 +87,166 @@ __device__ __forceinline__ uint32_t map_to_cta(uint32_t local_addr, uint32_t ran
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
   return r;
 }
-// Arrive on a barrier of another CTA of the cluster (the peer's epilogue warps hand the accumulator back to the leader's MMA
-// warp).  Default semantics (.release at CTA scope), like CUTLASS's ClusterBarrier::arrive(cta_id): what the waiter depends on
-// is the completion of this warp's tcgen05.ld (tcgen05.wait::ld + tcgen05.fence::before_thread_sync precede the arrive), not
-// the visibility of its global stores.  The former `.release.cluster` form compiled to MEMBAR.ALL.GPU + ERRBAR in front of
-// every arrive: each epilogue warp waited for its output stores to become GPU-visible once per tile -- 34 % of all stall
-// samples of flow_conv0@L0 (source-level ncu, profiles/r2i_stalls_flow_L0.md).
+// Arrive on a barrier of another CTA of the cluster.  Release at cluster scope: the arrive tells the peer's producer that
+// this warpgroup's wgmma reading the slot have retired, before the peer multicasts the next tap into it.
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
 }
-__device__ __forceinline__ void tma_load_4d_2sm(uint32_t dst, const CUtensorMap* tm, uint32_t leader_bar, int c0,
-                                                int c1, int c2, int c3) {
+
+// L2 prefetch of a 4-D tile (no smem destination, no barrier): hides DRAM latency for data that a
+// later cp.async.bulk.tensor of the same box will fetch.
+__device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* tm, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile [%0, {%1, %2, %3, %4}];" ::"l"(tm), "r"(c0),
+               "r"(c1), "r"(c2), "r"(c3)
+               : "memory");
+}
+
+// K-major swizzled shared-memory matrix descriptor of wgmma: start>>4 [0,14), LBO>>4 [16,30) (unused for
+// swizzled K-major, 1), SBO>>4 [32,46) = bytes between 8-row groups, base_offset [49,52) = 0,
+// layout [62,64) = 1 (SWIZZLE_128B, KC = 64: 128-byte rows) or 2 (SWIZZLE_64B, KC = 32: 64-byte rows).
+// The swizzle XOR acts on absolute smem address bits, so a start address at any 128 B (64 B) row and an SBO that
+// is not a multiple of the swizzle atom (the rows of a 10-pixel-wide halo box) address the TMA-written box directly.
+template <int KC>
+__device__ __forceinline__ uint64_t make_desc_sbo(uint32_t saddr, uint32_t sbo_bytes) {
+  constexpr uint64_t kType = (KC == 64) ? 1 : 2;
+  uint64_t d = 0;
+  d |= (uint64_t)((saddr & 0x3FFFFu) >> 4);
+  d |= (uint64_t)1 << 16;
+  d |= (uint64_t)(sbo_bytes >> 4) << 32;
+  d |= kType << 62;
+  return d;
+}
+// dense boxes: 8-row groups are one swizzle atom apart (1024 B for 128-byte rows, 512 B for 64-byte rows)
+template <int KC>
+__device__ __forceinline__ uint64_t make_desc_kc(uint32_t saddr) {
+  return make_desc_sbo<KC>(saddr, KC == 64 ? 1024u : 512u);
+}
+
+// Position in an mbarrier ring whose depth is a RUNTIME value: stage index + phase bit, advanced by
+// compare-and-wrap (`i % depth`, `(i / depth) & 1` compile to a long I2F / MUFU.RCP / F2I sequence per use).
+struct RingPos {
+  int stage = 0;
+  uint32_t phase = 0;
+  __device__ __forceinline__ void advance(int depth) {
+    if (++stage == depth) {
+      stage = 0;
+      phase ^= 1u;
+    }
+  }
+};
+
+// Division by a kernel-invariant divisor without the I2F / MUFU.RCP / IABS sequence of a runtime `/`:
+// q = (x * ceil(2^40 / d)) >> 40 is exact whenever x * d < 2^40 (tile indices and tile counts are < 2^20 for every frame
+// this engine accepts); otherwise the plain division is used.  The per-tile decode tile -> (b, y0, x0) runs in the
+// producer and every consumer warp for every tile.
+struct FastDiv {
+  uint64_t mul;
+  uint32_t d;
+  bool fast;
+  __device__ __forceinline__ FastDiv(int divisor, int max_x) : d((uint32_t)divisor) {
+    fast = (uint64_t)(uint32_t)max_x * d < (1ull << 40);
+    mul = ((1ull << 40) + d - 1) / d;
+  }
+  __device__ __forceinline__ void divmod(int x, int& q, int& r) const {
+    const uint32_t qq = fast ? (uint32_t)(((uint64_t)(uint32_t)x * mul) >> 40) : (uint32_t)x / d;
+    q = (int)qq;
+    r = x - (int)(qq * d);
+  }
+};
+
+// Warp-uniform leader election: the producer warp's role loop runs converged on all 32 lanes and one elected lane
+// issues the TMA instructions.
+__device__ __forceinline__ bool elect_one() {
+  uint32_t pred;
   asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(tm), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
+      "{\n\t.reg .pred P;\n\t"
+      "elect.sync _|P, 0xffffffff;\n\t"
+      "selp.u32 %0, 1, 0, P;\n\t}"
+      : "=r"(pred));
+  return pred != 0;
 }
-__device__ __forceinline__ void tma_load_2d_2sm(uint32_t dst, const CUtensorMap* tm, uint32_t leader_bar, int c0,
-                                                int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes"
-      " [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(tm), "r"(leader_bar), "r"(c0), "r"(c1)
-      : "memory");
+
+// ---------------------------------------------------------------------------------------------
+// Warpgroup MMA.  D[64 x N] (+)= A[64 x 16] * B[N x 16]^T, A and B K-major in shared memory.  Accumulator fragment of
+// thread t of the warpgroup (warp w = t / 32, lane l): rows 16w + l/4 (registers 4j, 4j+1) and 16w + l/4 + 8
+// (4j+2, 4j+3), columns 8j + 2(l%4) + {0, 1}, j = 0 .. N/8-1.  Successive wgmma on the same accumulator registers
+// need no wgmma.fence between them only when they have the same shape, so every kernel issues one N per accumulator.
+// ---------------------------------------------------------------------------------------------
+#ifdef FILM_SPLIT_FP16
+#define FILM_WGMMA_AB "f16.f16"
+#else
+#define FILM_WGMMA_AB "bf16.bf16"
+#endif
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void umma_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
+// keeps the compiler from moving accumulator reads or writes across wgmma_fence / wgmma_wait
+template <int R>
+__device__ __forceinline__ void acc_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// Register reallocation between warpgroups (the producer warpgroup hands its registers to the consumers)
+template <int N>
+__device__ __forceinline__ void regs_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N));
+}
+template <int N>
+__device__ __forceinline__ void regs_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N));
+}
+
+// scale_d = 0: D = A * B (first product of a tile), 1: D += A * B
+template <int N>
+__device__ __forceinline__ void wgmma(float* d, uint64_t a, uint64_t b, uint32_t scale_d);
+template <>
+__device__ __forceinline__ void wgmma<32>(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32." FILM_WGMMA_AB " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(a), "l"(b), "r"(scale_d));
 }
-// arrives (once all prior MMAs of this thread completed) on the barrier at the same offset in both CTAs
-__device__ __forceinline__ void umma_commit_2sm_mc(uint32_t bar) {
+template <>
+__device__ __forceinline__ void wgmma<64>(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-      ::"r"(bar), "h"((uint16_t)3)
-      : "memory");
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32." FILM_WGMMA_AB " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(a), "l"(b), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
+template <>
+__device__ __forceinline__ void wgmma<128>(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32." FILM_WGMMA_AB " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// instruction descriptor with an explicit M (256 for cta_group::2)
-template <int BN, int BM>
-__device__ __forceinline__ uint32_t make_idesc_m() {
-#ifdef FILM_SPLIT_FP16
-  constexpr uint32_t fmt = 0;
-#else
-  constexpr uint32_t fmt = 1;
-#endif
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+template <>
+__device__ __forceinline__ void wgmma<256>(float* d, uint64_t a, uint64_t b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32." FILM_WGMMA_AB " "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a), "l"(b), "r"(scale_d));
 }
 
 }  // namespace tc

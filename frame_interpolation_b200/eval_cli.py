@@ -1,4 +1,4 @@
-"""Benchmark evaluator on the B200 engine -- TF-free counterpart of the reference's `eval/eval_cli.py:88-178`.
+"""Benchmark evaluator on the H100 engine -- TF-free counterpart of the reference's `eval/eval_cli.py:88-178`.
 
     python -m frame_interpolation_b200.eval_cli --triplets <dir> --model_path <weights.filmw> \
         --output_dir <out> [--max_examples N] [--metrics l1,l2,ssim,psnr] [--output_frames]

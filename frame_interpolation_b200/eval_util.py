@@ -1,4 +1,4 @@
-"""Frame scheduling and image I/O on top of the B200 `Interpolator` (SURVEY.md section 8f row 1).
+"""Frame scheduling and image I/O on top of the engine's `Interpolator`.
 
 Counterpart of the reference's `eval/util.py:29-153` without TensorFlow:
   read_image / write_image                    eval/util.py:29-59   (cv2 instead of tf.io)
@@ -6,7 +6,7 @@ Counterpart of the reference's `eval/util.py:29-153` without TensorFlow:
 The yielded sequence is the reference's: for every consecutive input pair the in-order
 traversal of the mid-point tree (first frame included, second excluded), then the last frame.
 
-When the interpolator is the untiled B200 engine, each pair's whole tree is evaluated by ONE
+When the interpolator is the untiled engine, each pair's whole tree is evaluated by ONE
 device-resident call (`Interpolator.interpolate_recursively`): intermediate frames never leave
 HBM, which removes the per-mid-frame H2D + D2H + sync the reference pays
 (eval/interpolator.py:171,176). Any other callable `(x0, x1, dt) -> mid` takes the generic path.

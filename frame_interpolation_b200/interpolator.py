@@ -1,4 +1,4 @@
-"""Drop-in for the reference's `eval/interpolator.py` on top of the B200 engine.
+"""Drop-in for the reference's `eval/interpolator.py` on top of the H100 engine.
 
 Same class name, constructor arguments, methods, argument meaning and error behaviour
 as `eval.interpolator.Interpolator` (reference eval/interpolator.py:129-209):
@@ -11,7 +11,7 @@ as `eval.interpolator.Interpolator` (reference eval/interpolator.py:129-209):
 a TF2 SavedModel directory; the string "synthetic" (or "synthetic:<seed>") selects the
 seeded synthetic Style-architecture weights used by the tests and benchmarks.
 
-All arithmetic runs in libfilm_b200.so (hand-written sm_100a kernels) through the C ABI
+All arithmetic runs in libfilm_b200.so (hand-written sm_90a kernels) through the C ABI
 of include/film_b200.h. No TensorFlow, no torch, no CPU fallback.
 """
 from __future__ import annotations
@@ -89,7 +89,7 @@ class _PinnedPool:
 
 
 class Interpolator:
-    """A class for generating interpolated frames between two input frames (B200 engine)."""
+    """A class for generating interpolated frames between two input frames (H100 engine)."""
 
     def __init__(self, model_path: str, align: Optional[int] = None,
                  block_shape: Optional[List[int]] = None, device: int = 0) -> None:

@@ -1,4 +1,4 @@
-"""Command line front end with the reference's flags (eval/interpolator_cli.py:85-121) on the B200 engine.
+"""Command line front end with the reference's flags (eval/interpolator_cli.py:85-121) on the H100 engine.
 
     python -m frame_interpolation_b200.interpolator_cli --pattern "photos" --model_path synthetic \
         --times_to_interpolate 3 [--align 64] [--block_height 2 --block_width 2] [--output_video --fps 30]

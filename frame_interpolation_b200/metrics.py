@@ -1,5 +1,5 @@
-"""Image-quality metrics of the reference's benchmark evaluator, TensorFlow-free
-(SURVEY.md section 8f row 4): `psnr` / `ssim` as used by losses/losses.py:103-113
+"""Image-quality metrics of the reference's benchmark evaluator, TensorFlow-free:
+`psnr` / `ssim` as used by losses/losses.py:103-113
 (`tf.image.psnr(max_val=1.0)`, `tf.image.ssim(max_val=1.0)` with TF's defaults: 11x11 Gaussian
 window, sigma 1.5, k1 = 0.01, k2 = 0.03, VALID windows, mean over channels and positions).
 Used for the PSNR-delta parity figure; inputs are (..., H, W, C) float arrays."""

@@ -1,6 +1,6 @@
 """Multi-GPU sharding of the FILM hot path (one process per GPU, torch.distributed).
 
-The path shards into independent units (SURVEY.md section 8e):
+The path shards into independent units:
 
 * frame pairs  -- `interpolate_pairs`: contiguous block partition of N independent
   (x0, x1) pairs over ranks, weights replicated, ONE all-gather of the outputs so every

@@ -94,7 +94,7 @@ def level_sizes(h: int, w: int) -> List[Tuple[int, int]]:
 def conv_macs(h: int, w: int) -> Dict[str, int]:
     """Multiply-accumulates of every Conv2D call site for ONE network call on a
     (padded) h x w frame pair, counted as kh*kw*Cin*Cout per output pixel on the
-    reference graph (no credit for algebraic shortcuts). SURVEY.md section 8(d)."""
+    reference graph (no credit for algebraic shortcuts)."""
     sizes = level_sizes(h, w)
     fe = 0
     for i in range(PYRAMID_LEVELS):

@@ -1,4 +1,4 @@
-"""Seeded synthetic frame pairs (SURVEY.md section 8d).
+"""Seeded synthetic frame pairs.
 
 Not white noise (flow would be undefined and warps degenerate): a band-limited
 texture (sum of random-phase sinusoids per channel) rescaled to [0.05, 0.95];

@@ -2,7 +2,7 @@
 `variables/variables.index` + `variables/variables.data-00000-of-00001` pair inside a TF2
 SavedModel directory such as the released `pretrained_models/film_net/Style/saved_model`
 (reference README.md:69-83, written by training/train_lib.py:280 /
-training/build_saved_model_cli.py:73). SURVEY.md section 8f row 2.
+training/build_saved_model_cli.py:73).
 
 Format (tensorflow/core/util/tensor_bundle, tensorflow/core/lib/io/table -- a LevelDB-style
 sorted string table):

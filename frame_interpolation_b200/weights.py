@@ -10,9 +10,8 @@ Tensor names and shapes are `spec.weight_table()`: Keras HWIO kernels + biases,
 named after the reference's layers (`feature_extractor.py:118-123`,
 `pyramid_flow_estimator.py:76-83,115,119`, `fusion.py:76-101`).
 
-There is no pre-trained SavedModel and no TensorFlow in the build container
-(SURVEY.md section 8c), so tests and benchmarks use `synthetic_weights()`: seeded
-He-scaled tensors tuned so activations stay O(1) and level-0 flows are a few pixels
+No pre-trained SavedModel or TensorFlow is needed by the tests and benchmarks: they use
+`synthetic_weights()`, seeded He-scaled tensors tuned so activations stay O(1) and level-0 flows are a few pixels
 (otherwise the warps would be degenerate and parity vacuous). `from_named_arrays()`
 is the import hook for real weights (a dict of numpy arrays keyed by the SavedModel
 variable names, e.g. from `tf.train.load_checkpoint` on a machine that has TF).

@@ -1,5 +1,5 @@
 /*
- * film_b200.h -- C ABI of the B200-native FILM inference engine (libfilm_b200.so).
+ * film_b200.h -- C ABI of the H100-native (sm_90a) FILM inference engine (libfilm_b200.so).
  *
  * Drop-in boundary: every entry point replaces one piece of the reference's Python
  * inference wrapper, `eval/interpolator.py` (google-research/frame-interpolation):
@@ -28,7 +28,7 @@
  * a human-readable message for the last non-zero status on that handle (or on
  * creation, when handle is NULL).
  *
- * There is no CPU fallback: every entry point fails with status 2 if no sm_100
+ * There is no CPU fallback: every entry point fails with status 2 if no sm_90
  * device is present.
  *
  * Threading: a handle owns one CUDA stream, its per-shape plans (activation arenas, CUDA
@@ -135,7 +135,7 @@ FILM_API int film_synchronize(film_handle* h);
 FILM_API int film_profile(film_handle* h, film_profile_t* out);
 
 /* Engine options, set before the first call of a given shape.
- *   "conv_impl"   : 0 = tcgen05 implicit-GEMM kernels (default, the product path),
+ *   "conv_impl"   : 0 = wgmma implicit-GEMM kernels (default, the product path),
  *                   1 = fp32 CUDA-core validation kernels (debug only; used by the
  *                       tests to cross-check the tensor-core path on the device)
  *   "use_graph"   : 1 = capture each shape's schedule in a CUDA graph (default), 0 = eager
@@ -143,22 +143,19 @@ FILM_API int film_profile(film_handle* h, film_profile_t* out);
  *                   return it after the call; 0 (default) = activation buffers are recycled inside a plan
  *   "time_ops"    : 1 = run eagerly with one CUDA-event pair per kernel (see film_op_table)
  *   "conv3x3_v2"  : 1 = persistent tap-reuse kernel for 3x3 convs (default), 0 = generic kernel
- *   "conv3x3_2cta": 1 = CTA-pair (tcgen05 cta_group::2, M = 256) kernel for the streamed-weight 3x3
- *                   convs of the large pyramid levels (default), 0 = off, 2 = every eligible layer
- *   "conv3x3_halo": wide halo boxes -- one (64 ch, 10 px, 18 rows) TMA box per chunk serves all nine taps
- *                   (UMMA descriptors at pixel offsets): 3 = both persistent kernels, 64- and 32-channel chunks
- *                   (default: validated on hardware in round 2, -0.6 % / -2.0 % step time in two same-box A/Bs),
- *                   2 = 64-channel chunks only, 1 = CTA-pair kernel only, 0 = three dx-shifted 8-px boxes
+ *   "conv3x3_2cta": 1 = the streamed-weight 3x3 convs of the large pyramid levels run as (2,1,1) CTA clusters in which
+ *                   each CTA loads half of every weight tap and TMA-multicasts it to both, 0 = off (default: the
+ *                   paired layers measure slower on H100), 2 = every eligible layer
+ *   "conv3x3_halo": wide halo boxes of the persistent kernel -- one (64 ch, 10 px, 18 rows) TMA box per chunk serves all
+ *                   nine taps (wgmma descriptors at pixel offsets): 3 = 64- and 32-channel chunks (default),
+ *                   2 = 64-channel chunks only, 1 = CTA-pair layers only, 0 = three dx-shifted 8-px boxes
  *   "fe_conv0_tc" : cfeat_conv_0 (3 -> 64, K = 27): 0 = register-tiled fp32 FMA kernel reading the fp32 image directly
  *                   (default: exact fp32 arithmetic, no widened image tensor), 1 = tensor-core kernel over a 32-channel-
- *                   padded split image (0.78 ms against 0.87 ms over the seven levels in per-op timing)
- *   "conv3x3_dual": 1 = the CTA-pair kernel serves TWO spatial work items per streamed weight tap (both items' halo boxes
- *                   resident, two accumulator sets in TMEM): halves the weight bytes pulled from L2 per item on the
- *                   layers that are L2->SM ingest bound (default); 0 = one item per weight pass
+ *                   padded split image
  *   "plane_skip"  : 1 = lo planes that no consumer reads (destinations of single-pass convs) are neither gathered nor
  *                   written (default), 0 = always both planes
- *   "mma_straight": 1 = with resident weights one elected lane issues a whole activation stage as straight-line code
- *                   (default), 0 = per-tap issue loop
+ *   "mma_straight": 1 = with resident weights each warpgroup issues a whole activation stage as one wgmma group of
+ *                   straight-line code (default), 0 = one wgmma group per tap
  *   "arena_reuse" : 1 = activation buffers are recycled inside a plan by liveness (default), 0 = one buffer per tensor
  *   "fuse_flow_head": 1 = on flow level 0 (32-filter predictor) conv_3, conv_4 and the residual add run in the epilogue of
  *                   conv_2 (default), 2 = also on level 1 (64 filters: measured epilogue-bound, slower), 0 = separate launch
@@ -171,7 +168,7 @@ FILM_API int film_profile(film_handle* h, film_profile_t* out);
  *                   drop-and-retry before FILM_ERR_CUDA is returned. */
 /*   "onepass_mask": precision plan -- bit s selects the single-pass product (A_hi x W_hi, fp16 operands, fp32
  *                   accumulate) for stage s (film_stage_count / film_stage_name); every other conv runs the
- *                   three-pass split product.  The default is the measured plan of DESIGN.md section 3;
+ *                   three-pass split product.  The default is a measured per-stage plan;
  *                   0 = every conv three-pass (fp32-grade).  "onepass_default" (any value) restores it. */
 FILM_API int film_set_option(film_handle* h, const char* name, int value);
 /* Reads back an integer option ("onepass_mask", "onepass_default", "conv3x3_halo", "conv3x3_2cta", "keep_debug"). */
@@ -188,7 +185,7 @@ FILM_API int film_stage_name(int stage, char* buf, int buf_size);
 FILM_API int film_debug_read(film_handle* h, const char* name, float* dst, int64_t* count);
 
 /* Per-op table of the plan used by the last call, as CSV text
- * "idx,category,name,ms,ref_flops,alg_bytes" (category 0 = tcgen05 conv, 1 = warp gather,
+ * "idx,category,name,ms,ref_flops,alg_bytes" (category 0 = tensor-core conv, 1 = warp gather,
  * 2 = other bandwidth kernels). `ms` is filled by calls made with option "time_ops" = 1
  * (eager run, one CUDA event pair per kernel on the launching stream), else -1.
  * *needed receives the buffer size required. */
@@ -196,7 +193,7 @@ FILM_API int film_op_table(film_handle* h, char* buf, int64_t buf_size, int64_t*
 
 FILM_API const char* film_last_error(film_handle* h);
 
-/* Version / build info string: "film_b200 <ver> sm_100a split=fp16x2 mma=...". */
+/* Version / build info string: "film_b200 <ver> sm_90a split=fp16x2 mma=...". */
 FILM_API const char* film_version(void);
 
 #ifdef __cplusplus

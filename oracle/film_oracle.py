@@ -4,8 +4,8 @@ Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl refere
 legs may import this module. The engine (frame_interpolation_b200/) never does and has
 no CPU fallback.
 
-PARITY UNPINNED: the reference ships no unit tests and no golden vectors (SURVEY.md
-section 4), and its arithmetic lives in un-vendored third-party packages that are absent
+PARITY UNPINNED: the reference ships no unit tests and no golden vectors, and its arithmetic
+lives in un-vendored third-party packages that are absent
 from this image -- tensorflow==2.6.2 and tensorflow-addons==0.15.0 (reference
 requirements.txt:2,4) -- and no pre-trained SavedModel exists on disk. This file is an
 op-for-op restatement of the reference graph in PyTorch-CPU with the TF / TFA op semantics

@@ -1,5 +1,5 @@
 """Generates tests/golden/*.npz from the CPU oracle (the reference itself cannot run here:
-no TensorFlow, no SavedModel -- SURVEY.md section 8c -- so these vectors pin the ORACLE, i.e.
+no TensorFlow, no SavedModel -- so these vectors pin the ORACLE, i.e.
 they guard the restatement against accidental change and give the GPU tests fixed targets).
 
     python tests/golden/make_golden.py

@@ -1,6 +1,6 @@
 """A second, independently written restatement of the reference graph -- pure numpy, explicit tap sums and index arithmetic,
 no torch ops -- checked against `oracle/film_oracle.py` on a 64x64 frame pair. The two share nothing but the weight table:
-if either mis-states a TF / TFA rule of SURVEY.md section 8c (SAME padding asymmetry of the 2x2 conv, VALID pooling, half-pixel
+if either mis-states a TF / TFA rule of the reference graph (SAME padding asymmetry of the 2x2 conv, VALID pooling, half-pixel
 bilinear resize of `2 * v`, NEAREST resize, TFA's clamp-then-lerp warp with the (dy, dx) flip, concat orders, predictor
 indexing, flow scaling by 0.5), the outputs diverge. This does not pin the oracle to TensorFlow (nothing offline can); it
 removes "one author's reading of torch semantics" as a single point of failure."""

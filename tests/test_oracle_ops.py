@@ -1,5 +1,5 @@
-"""Closed-form checks of the third-party op semantics the oracle restates
-(SURVEY.md section 8c rules 1-7). CPU only."""
+"""Closed-form checks of the third-party op semantics the oracle restates (TF SAME / VALID padding, half-pixel bilinear
+and NEAREST resize, TFA dense_image_warp with its border clamp, concat orders). CPU only."""
 import numpy as np
 import pytest
 import torch

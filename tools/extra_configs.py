@@ -1,4 +1,4 @@
-"""BASELINE.json configs[2..4] on one B200 through the public API (host buffers): 4K tiled 2x2,
+"""BASELINE.json configs[2..4] on one H100 through the public API (host buffers): 4K tiled 2x2,
 720p recursive times_to_interpolate=6 (63 mid-frames, device-resident recursion), 8K tiled 4x4."""
 import json, os, sys, time
 import numpy as np
