@@ -21,6 +21,8 @@ SOURCES = ["film_engine.cu", "film_kernels.cu", "film_conv_tc.cu", "film_conv3x3
 HEADERS = ["film_common.cuh", "film_conv.h", "film_kernels.h", "film_tc_ptx.cuh", os.path.join("..", "..", "include", "film_b200.h")]
 LIB = os.path.join(HERE, "libfilm_b200.so")
 STAMP = os.path.join(HERE, "_build", "stamp")
+# ptxas remark (C75xx) for a kernel whose wgmma instructions it had to serialise; the build fails on it
+SERIALIZED = "wgmma.mma_async instructions are serialized"
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
@@ -68,12 +70,17 @@ def build(force: bool = False, verbose: bool = False) -> str:
         objs.append(obj)
         cmd = [nvcc, *flags, "-c", os.path.join(CSRC, src), "-o", obj]
         procs.append((cmd, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
+    serialized = []
     for cmd, p in procs:
         out, _ = p.communicate()
         if verbose or p.returncode:
             sys.stderr.write(out)
         if p.returncode:
             raise RuntimeError("nvcc failed: " + " ".join(cmd))
+        serialized += [ln for ln in out.splitlines() if SERIALIZED in ln]
+    if serialized:
+        # ptxas let each wgmma wait for the previous one to finish: a silent loss of most of the tensor-core rate
+        raise RuntimeError("ptxas serialised wgmma:\n" + "\n".join(serialized))
     link = [nvcc, "-shared", "-o", LIB, *objs, "-cudart", "static", "-Xlinker", "-z,defs", "-lpthread", "-ldl", "-lrt"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if verbose or r.returncode:

@@ -30,9 +30,6 @@ struct ConvSrc {
   int bswap;   // 1: this source is read with the batch index swapped (b -> B - 1 - b): the coarsest flow level pairs
                // the features of image 0 with the UNWARPED features of image 1 and vice versa
                // (pyramid_flow_estimator.py:148-149), which is the same tensor at the other batch index
-  int ksteps;  // 16-channel k-steps issued per chunk (< kchunk/16 when the tail channels of every chunk are
-               // zero padding, e.g. the 10-of-64 "side" source): skipping is exact.  Honoured by the persistent
-               // 3x3 kernels; the generic kernel issues every k-step
 };
 
 struct alignas(64) ConvProblem {
@@ -87,6 +84,10 @@ struct alignas(64) ConvProblem {
   int v2_resident;        // 1: all W_hi/W_lo K blocks stay in shared memory for the CTA's lifetime
   int v2_na, v2_nw;       // activation-ring / weight-ring stages
   int v2_grid;            // persistent CTAs
+  int v2_part_lo, v2_part_hi;  // activation stages [lo, hi) of every tile read the one source whose chunks hold data in
+                               // their first 16-channel k-step only (the 10-of-64 "side" source, the 3-of-32 image
+                               // block): the kernel issues that k-step alone there, skipping the zero padding exactly.
+                               // lo == hi: no such source.  The generic kernel issues every k-step
   // optional fused 2x2/2 average pool of the (activated, fp32) output tile, written as a second
   // split tensor [B][H/2][W/2][pool_C] (feature_extractor.py:138-146); null = off
   sp_t* pool_hi;

@@ -57,10 +57,11 @@ constexpr int kHeadBytes = kHeadW3 + kHeadMisc;
 
 __host__ __device__ inline int w_tap_bytes(int bn, int kc, int planes = 2) { return bn * kc * 2 * planes; }  // [BN x KC] hi (+ lo)
 
-// Variants are template parameters chosen on the host (launch_conv3x3_tc): kPartial = some source's trailing 16-channel
-// k-steps are zero padding in every chunk (ConvSrc::ksteps < KC/16: the 10-of-64 "side" source, the 3-of-32 image
-// block) and are skipped; kHalo = wide halo boxes; kOne = single-pass product A_hi x W_hi (hi planes only);
-// kRes = resident weights issued as straight-line code (a whole activation stage is one wgmma group).
+// Variants are template parameters chosen on the host (launch_conv3x3_tc): kPartial = the activation stages
+// [v2_part_lo, v2_part_hi) of every tile read a source whose chunks hold data in their first 16-channel k-step only (the
+// 10-of-64 "side" source, the 3-of-32 image block); the all-zero k-steps are skipped; kHalo = wide halo boxes; kOne =
+// single-pass product A_hi x W_hi (hi planes only); kRes = resident weights issued as straight-line code (a whole
+// activation stage is one wgmma group).
 template <int BN, int KC, bool kPartial, bool kHalo, bool kOne, bool kRes>
 __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* __restrict__ prob) {
   extern __shared__ uint8_t smem_raw[];
@@ -127,8 +128,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
     for (int s = 0; s < kMaxSrc; ++s) {
       src_tab[2 * s] = s < nsrc ? prob->src[s].nchunk : 0;
       src_tab[2 * s + 1] = s < nsrc ? prob->src[s].c_off : 0;
-      src_tab[2 * kMaxSrc + s] = s < nsrc ? prob->src[s].ksteps : 0;
-      src_tab[3 * kMaxSrc + s] = s < nsrc ? prob->src[s].bswap : 0;
+      src_tab[2 * kMaxSrc + s] = s < nsrc ? prob->src[s].bswap : 0;
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -193,7 +193,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
       int kb = 0;
       for (int s = 0; s < nsrc; ++s) {
         const int nchunk = src_tab[2 * s], c_off = src_tab[2 * s + 1];
-        const int bs = src_tab[3 * kMaxSrc + s] ? prob->B - 1 - b : b;
+        const int bs = src_tab[2 * kMaxSrc + s] ? prob->B - 1 - b : b;
         const CUtensorMap* tm_hi = &prob->tm_a_hi[s];
         const CUtensorMap* tm_lo = &prob->tm_a_lo[s];
         for (int ch = 0; ch < nchunk; ++ch) {
@@ -288,9 +288,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
   {
     constexpr int kWTapC = kWPlane * (kOne ? 1 : 2);
     constexpr int kStageTaps = kHalo ? 9 : 3;   // taps served by one activation stage
-    constexpr int kSrcStages = kHalo ? 1 : 3;   // activation stages per chunk
     constexpr uint32_t kPx = KC * 2;            // bytes of one pixel row of a box
     const int nab = nkb / kStageTaps;           // activation stages per tile
+    [[maybe_unused]] const int part_lo = prob->v2_part_lo, part_hi = prob->v2_part_hi;   // kPartial: 1-k-step stages
     // first pixel row of this warpgroup's 64 pixels inside the box, and the stride between its 8-row groups
     const uint32_t a_row0 = kHalo ? (uint32_t)(wg * 8 * kHaloW) * kPx : (uint32_t)(wg * 64) * kPx;
     const uint32_t sbo = kHalo ? kHaloW * kPx : 8 * kPx;
@@ -309,17 +309,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
         rel_a = next_a;
         rel_w = next_w;
       };
-      [[maybe_unused]] int src_i = 0, src_left = src_tab[0] * kSrcStages;  // stages left in the current source
-      for (int ab = 0; ab < nab; ++ab) {
-        [[maybe_unused]] int ksteps = KC / 16;
-        if constexpr (kPartial) {
-          while (src_left == 0) {
-            ++src_i;
-            src_left = src_tab[2 * src_i] * kSrcStages;
-          }
-          --src_left;
-          ksteps = src_tab[2 * kMaxSrc + src_i];
-        }
+      // One activation stage whose products each issue kSteps k-steps (a compile-time count: ptxas serialises every
+      // wgmma of a kernel in which a runtime condition picks between wgmma sequences, C7520)
+      auto stage = [&](auto ksteps_c) {
+        constexpr int kSteps = decltype(ksteps_c)::value;
         const int st = ra.stage;
         mbar_wait(tail + 8u * st, ra.phase);
         const uint32_t sa = a_base + st * kAStage + a_row0;
@@ -339,21 +332,19 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
             const uint64_t a_lo = a_hi + lo_delta;
             const uint64_t w_hi = w0 + (uint64_t)((t * kWTapC) >> 4), w_lo = w_hi + (uint64_t)(kWPlane >> 4);
 #pragma unroll
-            for (int k = 0; k < KC / 16; ++k) {
-              if (!kPartial || k < ksteps) {
-                const uint64_t adv = (uint64_t)(k * 32 >> 4);
-                const uint32_t accf = (t == 0 && k == 0) ? first : 1u;
-                if constexpr (kOne) {
-                  wgmma<BN>(acc, a_hi + adv, w_hi + adv, accf);
-                } else if constexpr (kFused) {
-                  wgmma<BN>(acc, a_hi + adv, w_hi + adv, accf);
-                  wgmma<BN>(acc + BN / 2, a_hi + adv, w_lo + adv, accf);
-                  wgmma<BN>(acc, a_lo + adv, w_hi + adv, 1u);
-                } else {
-                  wgmma<BN>(acc, a_lo + adv, w_hi + adv, accf);
-                  wgmma<BN>(acc, a_hi + adv, w_lo + adv, 1u);
-                  wgmma<BN>(acc, a_hi + adv, w_hi + adv, 1u);
-                }
+            for (int k = 0; k < kSteps; ++k) {
+              const uint64_t adv = (uint64_t)(k * 32 >> 4);
+              const uint32_t accf = (t == 0 && k == 0) ? first : 1u;
+              if constexpr (kOne) {
+                wgmma<BN>(acc, a_hi + adv, w_hi + adv, accf);
+              } else if constexpr (kFused) {
+                wgmma<BN>(acc, a_hi + adv, w_hi + adv, accf);
+                wgmma<BN>(acc + BN / 2, a_hi + adv, w_lo + adv, accf);
+                wgmma<BN>(acc, a_lo + adv, w_hi + adv, 1u);
+              } else {
+                wgmma<BN>(acc, a_lo + adv, w_hi + adv, accf);
+                wgmma<BN>(acc, a_hi + adv, w_lo + adv, 1u);
+                wgmma<BN>(acc, a_hi + adv, w_hi + adv, 1u);
               }
             }
           }
@@ -377,10 +368,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
             const uint32_t first = (kb == 0) ? 0u : 1u;
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < KC / 16; ++k) {
-              if constexpr (kPartial) {
-                if (k >= ksteps) break;
-              }
+            for (int k = 0; k < kSteps; ++k) {
               const uint64_t adv = (uint64_t)(k * 32 >> 4);
               if constexpr (kOne) {
                 wgmma<BN>(acc, a_hi + adv, w_hi + adv, k == 0 ? first : 1u);
@@ -399,6 +387,15 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
           }
         }
         ra.advance(NA);
+      };
+      // the partial source's stages run in a loop of their own: no condition between alternative wgmma sequences
+      using Full = std::integral_constant<int, KC / 16>;
+      if constexpr (kPartial) {
+        for (int ab = 0; ab < part_lo; ++ab) stage(Full{});
+        for (int ab = part_lo; ab < part_hi; ++ab) stage(std::integral_constant<int, 1>{});
+        for (int ab = part_hi; ab < nab; ++ab) stage(Full{});
+      } else {
+        for (int ab = 0; ab < nab; ++ab) stage(Full{});
       }
       wgmma_wait<0>();
       if (is_leader) {
@@ -675,8 +672,7 @@ struct Variants {
   }
   static cudaError_t launch(const ConvProblem* d_prob, const ConvProblem& h, cudaStream_t st) {
     if (h.v2_na < 2 || (!h.v2_resident && h.v2_nw < 2)) return cudaErrorInvalidValue;   // see ring_depths
-    bool partial = false;
-    for (int s = 0; s < h.nsrc; ++s) partial |= h.src[s].nchunk > 0 && h.src[s].ksteps < KC / 16;
+    const bool partial = h.v2_part_hi > h.v2_part_lo;
     const int idx = (partial ? 8 : 0) | (h.halo ? 4 : 0) | (h.passes == 1 ? 2 : 0) | (h.v2_resident && h.straight ? 1 : 0);
     if (!h.pair) {
       kFn[idx]<<<h.v2_grid, kThreads, smem_bytes_for(h, BN), st>>>(d_prob);

@@ -624,7 +624,6 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
     cp.src[s].C = b->C;
     cp.src[s].c_off = sources[s].c_off;
     cp.src[s].nchunk = pc.src_chunks[s];
-    cp.src[s].ksteps = pc.src_ksteps[s];
     cp.src[s].bswap = sources[s].bswap;
     if (sources[s].c_off + pc.src_chunks[s] * kc > b->C) throw Error{FILM_ERR_ARG, "conv source channel overrun"};
     make_act_map(&cp.tm_a_hi[s], b->hi, b->B, b->H, b->W, b->C, box_h, box_w, kc);
@@ -697,6 +696,19 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
       const SplitBuf* b = sources[s].buf;
       make_act_map(&cp.tm_a_hi[s], b->hi, b->B, b->H, b->W, b->C, box_h, box_w + 2, kc);
       make_act_map(&cp.tm_a_lo[s], b->lo, b->B, b->H, b->W, b->C, box_h, box_w + 2, kc);
+    }
+  }
+  if (v2) {
+    // the activation stages of a source with all-zero k-steps (one halo box or three dx boxes per chunk); the kernel
+    // runs them in a loop of their own that issues the first k-step only
+    const int nst = cp.halo ? 1 : 3;
+    for (int s = 0, ab = 0; s < cp.nsrc; ab += pc.src_chunks[s] * nst, ++s) {
+      if (pc.src_chunks[s] == 0 || pc.src_ksteps[s] == kc / 16) continue;
+      if (pc.src_ksteps[s] != 1 || cp.v2_part_hi > cp.v2_part_lo)
+        throw Error{FILM_ERR_UNSUPPORTED, "persistent 3x3 conv: only one source may skip k-steps, and it must issue one (" +
+                                              tag + ")"};
+      cp.v2_part_lo = ab;
+      cp.v2_part_hi = ab + pc.src_chunks[s] * nst;
     }
   }
   const size_t idx = P.h_probs.size();
