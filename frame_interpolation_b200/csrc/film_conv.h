@@ -42,7 +42,7 @@ struct alignas(64) ConvProblem {
   ConvSrc src[kMaxSrc];
   int nsrc;
   int B, H, W;              // GEMM-M grid == input grid
-  int tile_h, tile_w;       // tile_h * tile_w == 128
+  int tile_h, tile_w;       // tile_h * tile_w == 128 (256: persistent kernel with pxn)
   int tiles_y, tiles_x;
   int ntaps;
   int tap_dy[kMaxTaps], tap_dx[kMaxTaps];
@@ -79,8 +79,9 @@ struct alignas(64) ConvProblem {
   const float* head_vup;  // [B][H][W][2] or null (coarsest level)
   float* head_res;        // [B][H][W][2]
   float* head_v;          // [B][H][W][2]
-  // persistent 3x3 kernel (film_conv3x3_tc.cu): tile is fixed 16 x 8, taps are dx-major,
-  // tm_a_* boxes are (64 ch, 8 px, 18 rows).  Pipeline shape chosen on the host:
+  // persistent 3x3 kernel (film_conv3x3_tc.cu): tiles of 128 pixels (16 x 8, 8 x 16 or 4 x 32; 32 x 8 = 256 pixels
+  // with pxn), taps are dx-major, tm_a_* boxes are (KC ch, tile_w px, tile_h + 2 rows), or tile_w + 2 px wide with
+  // `halo`.  Pipeline shape chosen on the host:
   int v2_resident;        // 1: all W_hi/W_lo K blocks stay in shared memory for the CTA's lifetime
   int v2_na, v2_nw;       // activation-ring / weight-ring stages
   int v2_grid;            // persistent CTAs
@@ -107,6 +108,8 @@ struct alignas(64) ConvProblem {
   int straight;           // persistent kernel, resident weights: 1 = a whole activation stage is one wgmma group issued as
                           // straight-line code (default), 0 = one group per tap
   int out_lo_skip;        // 1: every consumer of the destination reads the hi plane only -> the lo plane is not written
+  int pxn;                // persistent kernel, Cout = 64, 64-channel chunks, store / pool epilogue: 1 = pixels on the wgmma N
+                          // dimension (D^T = W_tap x A^T, m64n128k16, 32x8 tiles of 128 pixels per consumer warpgroup)
 };
 
 // launchers (film_conv_tc.cu / film_kernels.cu)

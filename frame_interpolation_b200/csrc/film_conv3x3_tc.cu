@@ -14,10 +14,18 @@
 //    the consumers drain the accumulators of the current one.
 //  * Two-accumulator product (BN <= 128): A_hi x W_hi and A_lo x W_hi accumulate into columns [0, BN) and A_hi x W_lo
 //    into columns [BN, 2 BN) of one register accumulator, all as N = BN wgmma; the epilogue adds the halves.
+//  * Pixels on N (kPxN: Cout = 64, 64-channel chunks): a Cout = 64 layer would issue m64n64k16 with both operands read
+//    from shared memory, 4 KiB of operand reads per 64x64x16 MACs.  This form computes D^T = W_tap x A^T instead: the
+//    weight tap [64 x 64] is the A operand, the activation box the B operand, and each consumer warpgroup owns 128
+//    pixels (16 tile rows of 8) of a 32x8 tile, so every product is one m64n128k16 (3 KiB per 64x64x16 MACs, the
+//    ratio of the BN = 128 layers) and each weight tap serves 256 pixels.  The three products of the three-pass form
+//    share one accumulator.  The transposed accumulator holds couts on its rows: the epilogue stages each plane
+//    through shared memory with stmatrix.trans and stores whole 128-byte pixels; the fused 2x2 pool finds its
+//    partners in the thread's own registers (column e ^ 1, row j + 1).
 //
 // Roles: warp 8 (warpgroup 2, registers handed to the consumers) = TMA producer (+ L2 prefetch of the next tile's boxes; warp-uniform, one elected lane issues),
-// warps 0-7 = two consumer warpgroups, each owning 64 pixels of the tile: wgmma into register accumulators, then the
-// epilogue straight from the registers.
+// warps 0-7 = two consumer warpgroups, each owning 64 (kPxN: 128) pixels of the tile: wgmma into register
+// accumulators, then the epilogue straight from the registers.
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -37,15 +45,15 @@ constexpr int kThreads = kConsumers + 128;   // + the producer warpgroup (one ac
 // 16x8 has the smallest halo (18/16); 8x16 and 4x32 exist to avoid wave quantisation on small levels.
 __host__ __device__ constexpr int a_plane_bytes(int kc, int th, int tw) { return (th + 2) * tw * kc * 2; }
 __host__ __device__ constexpr int a_stage_bytes(int kc, int th, int tw) { return 2 * a_plane_bytes(kc, th, tw); }
-// Wide-halo mode (16x8 tiles): ONE box (KC ch, 10 px, 18 rows) per plane and chunk serves all nine taps -- the
-// descriptor of tap (dy, dx) starts (dy * 10 + dx) pixel rows into the box and steps 10 pixel rows between 8-row
-// groups.  2.4x less L2 -> smem activation traffic than the three dx-shifted boxes.
-constexpr int kHaloW = 10, kHaloRows = 18;
-__host__ __device__ constexpr int halo_box_bytes(int kc) { return kHaloRows * kHaloW * kc * 2; }  // 23,040 for KC = 64
-__host__ __device__ constexpr int halo_plane_bytes(int kc) { return (halo_box_bytes(kc) + 1023) & ~1023; }  // 1 KiB-aligned planes
+// Wide-halo mode (16x8 tiles, 32x8 with kPxN): ONE box (KC ch, 10 px, tile_h + 2 rows) per plane and chunk serves all
+// nine taps -- the descriptor of tap (dy, dx) starts (dy * 10 + dx) pixel rows into the box and steps 10 pixel rows
+// between 8-row groups.  2.4x less L2 -> smem activation traffic than the three dx-shifted boxes.
+constexpr int kHaloW = 10;
+__host__ __device__ constexpr int halo_box_bytes(int kc, int th) { return (th + 2) * kHaloW * kc * 2; }  // 23,040 for KC = 64, 16 rows
+__host__ __device__ constexpr int halo_plane_bytes(int kc, int th) { return (halo_box_bytes(kc, th) + 1023) & ~1023; }  // 1 KiB-aligned planes
 // `planes` = 2 (hi + lo, three-pass product) or 1 (single-pass layers load the hi planes only)
 __host__ __device__ constexpr int a_stage_bytes_h(int kc, int th, int tw, int halo, int planes = 2) {
-  return planes * (halo ? halo_plane_bytes(kc) : a_plane_bytes(kc, th, tw));
+  return planes * (halo ? halo_plane_bytes(kc, th) : a_plane_bytes(kc, th, tw));
 }
 constexpr int kMaxRing = 8;
 constexpr int kSmemLimit = 227 * 1024;
@@ -54,6 +62,11 @@ constexpr int kFixedBytes = kBarBytes + 16 + 512 * 4 /*bias*/ + 64 /*src table: 
 // flow-head epilogue (epi_mode 3): W3 [64][32] + b3 / W4 / b4, after the src table
 constexpr int kHeadW3 = 64 * 32 * 4, kHeadMisc = 512;
 constexpr int kHeadBytes = kHeadW3 + kHeadMisc;
+// kPxN store epilogue, after the src table: per consumer warpgroup one plane of 64 pixels x 64 channels
+constexpr int kPxnStageWg = 64 * 64 * 2;
+constexpr int kPxnStageBytes = 2 * kPxnStageWg;
+// shared memory of the epilogue scratch after the src table
+inline int epi_scratch_bytes(int epi_mode, int pxn) { return epi_mode == 3 ? kHeadBytes : pxn ? kPxnStageBytes : 0; }
 
 __host__ __device__ inline int w_tap_bytes(int bn, int kc, int planes = 2) { return bn * kc * 2 * planes; }  // [BN x KC] hi (+ lo)
 
@@ -61,22 +74,25 @@ __host__ __device__ inline int w_tap_bytes(int bn, int kc, int planes = 2) { ret
 // [v2_part_lo, v2_part_hi) of every tile read a source whose chunks hold data in their first 16-channel k-step only (the
 // 10-of-64 "side" source, the 3-of-32 image block); the all-zero k-steps are skipped; kHalo = wide halo boxes; kOne =
 // single-pass product A_hi x W_hi (hi planes only); kRes = resident weights issued as straight-line code (a whole
-// activation stage is one wgmma group).
-template <int BN, int KC, bool kPartial, bool kHalo, bool kOne, bool kRes>
+// activation stage is one wgmma group); kPxN = pixels on N (BN = 64, KC = 64, 32x8 tiles, store / pool epilogue only).
+template <int BN, int KC, bool kPartial, bool kHalo, bool kOne, bool kRes, bool kPxN = false>
 __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* __restrict__ prob) {
+  static_assert(!kPxN || (BN == 64 && KC == 64), "pixels on N: Cout = 64 (one M = 64 weight tile), 64-channel chunks");
   extern __shared__ uint8_t smem_raw[];
   constexpr bool one = kOne;
   const int planes = one ? 1 : 2;
   constexpr int kWPlane = BN * KC * 2;  // one weight plane of one tap
   const int kWTap = kWPlane * planes;
   const int kTileH = prob->tile_h, kTileW = prob->tile_w;
-  constexpr int kHaloBox = halo_box_bytes(KC), kHaloPlane = halo_plane_bytes(KC);
-  constexpr bool halo = kHalo;   // plan guarantees 16x8 tiles
+  constexpr int kHaloTileH = kPxN ? 32 : 16;   // the only tile height of a wide-halo box
+  constexpr int kHaloBox = halo_box_bytes(KC, kHaloTileH), kHaloPlane = halo_plane_bytes(KC, kHaloTileH);
+  constexpr bool halo = kHalo;   // plan guarantees 16x8 (kPxN: 32x8) tiles
   const int kAPlane = halo ? kHaloPlane : a_plane_bytes(KC, kTileH, kTileW);
   const int kAStage = planes * kAPlane;
   const int kRowStep = kTileW * KC * 2;  // one tile row of pixels = tile_w/8 swizzle atoms
-  constexpr bool kFused = BN <= 128;
-  constexpr int kAccRegs = (kFused ? 2 * BN : BN) / 2;
+  constexpr bool kFused = BN <= 128 && !kPxN;
+  constexpr int kAccRegs = kPxN ? 64 : (kFused ? 2 * BN : BN) / 2;   // kPxN: m64n128 f32
+  constexpr int kWgPx = kPxN ? 128 : 64;                              // pixels per consumer warpgroup
 
   // ---- problem fields -> registers, once (the asm "memory" clobbers would otherwise force a
   //      global reload of every P.* access inside the role loops)
@@ -240,7 +256,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
 
   // ============================ consumer warpgroups: MMA + epilogue ============================
   regs_inc<232>();
-  const int wg = warp >> 2;        // pixels [64 wg, 64 wg + 64) of the tile
+  const int wg = warp >> 2;        // pixels [kWgPx wg, kWgPx (wg + 1)) of the tile
   const int q = lane & 3;
   const int H = prob->H, W = prob->W, out_H = prob->out_H, out_W = prob->out_W, out_C = prob->out_C;
   const int out_c_off = prob->out_c_off, act = prob->act;
@@ -291,8 +307,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
     constexpr uint32_t kPx = KC * 2;            // bytes of one pixel row of a box
     const int nab = nkb / kStageTaps;           // activation stages per tile
     [[maybe_unused]] const int part_lo = prob->v2_part_lo, part_hi = prob->v2_part_hi;   // kPartial: 1-k-step stages
-    // first pixel row of this warpgroup's 64 pixels inside the box, and the stride between its 8-row groups
-    const uint32_t a_row0 = kHalo ? (uint32_t)(wg * 8 * kHaloW) * kPx : (uint32_t)(wg * 64) * kPx;
+    // first pixel row of this warpgroup's pixels inside the box, and the stride between its 8-row groups
+    const uint32_t a_row0 = kHalo ? (uint32_t)(wg * (kWgPx / 8) * kHaloW) * kPx : (uint32_t)(wg * kWgPx) * kPx;
     const uint32_t sbo = kHalo ? kHaloW * kPx : 8 * kPx;
     RingPos ra, rw;   // activation / weight ring positions
     float acc[kAccRegs];
@@ -335,7 +351,13 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
             for (int k = 0; k < kSteps; ++k) {
               const uint64_t adv = (uint64_t)(k * 32 >> 4);
               const uint32_t accf = (t == 0 && k == 0) ? first : 1u;
-              if constexpr (kOne) {
+              if constexpr (kPxN) {   // D^T += W x A^T: the weight tap is the M = 64 operand
+                wgmma<128>(acc, w_hi + adv, a_hi + adv, accf);
+                if constexpr (!kOne) {
+                  wgmma<128>(acc, w_lo + adv, a_hi + adv, 1u);
+                  wgmma<128>(acc, w_hi + adv, a_lo + adv, 1u);
+                }
+              } else if constexpr (kOne) {
                 wgmma<BN>(acc, a_hi + adv, w_hi + adv, accf);
               } else if constexpr (kFused) {
                 wgmma<BN>(acc, a_hi + adv, w_hi + adv, accf);
@@ -370,7 +392,13 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
 #pragma unroll
             for (int k = 0; k < kSteps; ++k) {
               const uint64_t adv = (uint64_t)(k * 32 >> 4);
-              if constexpr (kOne) {
+              if constexpr (kPxN) {
+                wgmma<128>(acc, w_hi + adv, a_hi + adv, k == 0 ? first : 1u);
+                if constexpr (!kOne) {
+                  wgmma<128>(acc, w_lo + adv, a_hi + adv, 1u);
+                  wgmma<128>(acc, w_hi + adv, a_lo + adv, 1u);
+                }
+              } else if constexpr (kOne) {
                 wgmma<BN>(acc, a_hi + adv, w_hi + adv, k == 0 ? first : 1u);
               } else if constexpr (kFused) {
                 wgmma<BN>(acc, a_hi + adv, w_hi + adv, k == 0 ? first : 1u);
@@ -411,6 +439,83 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
       div_tx.divmod(rem, ty, tx);
       const int n0 = nti * BN;
       const bool live = sp < nsp;   // false: the empty partner of an odd tile count stores nothing
+      if constexpr (kPxN) {
+        // Transposed accumulator: register 4j + 2h + e holds cout c0 + 8h and pixel (tile row 16 wg + j, column 2q + e)
+        const int c0 = 16 * (warp & 3) + (lane >> 2);
+        const float bias0 = bias_smem[c0], bias1 = bias_smem[c0 + 8];
+#pragma unroll
+        for (int i = 0; i < kAccRegs; ++i) {
+          const float f = acc[i] + ((i & 2) ? bias1 : bias0);
+          acc[i] = act ? leaky(f) : f;
+        }
+        const int y_wg = ty * kTileH + 16 * wg, x_t = tx * kTileW;
+        if (do_pool) {
+          // 2x2 partners in the thread's own registers: the next column is e ^ 1, the next row is j + 1.  The lane of
+          // the odd cout (lane ^ 4) hands its sum over, and the even-cout lane stores the pair
+          const int px = x_t + 2 * q;
+#pragma unroll
+          for (int j = 0; j < 16; j += 2) {
+            const int py = y_wg + j;
+            const bool ok = live && py < H && px < W && !(lane & 4);
+            const int64_t ppix = ((int64_t)b * (out_H >> 1) + (py >> 1)) * (out_W >> 1) + (px >> 1);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int i = 4 * j + 2 * h;
+              const float v = ((acc[i] + acc[i + 1]) + (acc[i + 4] + acc[i + 5])) * 0.25f;
+              const float vn = __shfl_xor_sync(0xffffffffu, v, 4);
+              if (ok) {
+                uint32_t hi, lo;
+                split_pack2(v, vn, hi, lo);
+                *reinterpret_cast<uint32_t*>(pool_hi + ppix * pool_C + c0 + 8 * h) = hi;
+                *reinterpret_cast<uint32_t*>(pool_lo + ppix * pool_C + c0 + 8 * h) = lo;
+              }
+            }
+          }
+        }
+        // Split store: each plane goes through shared memory 64 pixels at a time.  stmatrix.trans writes 8 couts of one
+        // pixel as one 16-byte row (chunk cout / 8 of the pixel's 128 bytes, XOR-swizzled by pixel % 8: conflict-free);
+        // eight consecutive threads then store one pixel's 128 bytes
+        uint8_t* const stg = reinterpret_cast<uint8_t*>(src_tab) + 64 + wg * kPxnStageWg;
+        const uint32_t stg_u = smem_u32(stg);
+        const int t128 = threadIdx.x & 127;
+        auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); };
+        for (int pl = 0; pl < (lo_skip ? 1 : 2); ++pl) {
+          sp_t* const dst = pl ? out_lo : out_hi;
+#pragma unroll
+          for (int half = 0; half < 2; ++half) {
+            wg_sync();   // the previous round's reads are done
+#pragma unroll
+            for (int jj = 0; jj < 8; jj += 2) {
+              uint32_t r[4];   // matrices (j, h) = (jj, 0), (jj, 1), (jj + 1, 0), (jj + 1, 1)
+#pragma unroll
+              for (int m = 0; m < 4; ++m) {
+                const int i = 4 * (8 * half + jj + (m >> 1)) + 2 * (m & 1);
+                if (pl) {
+                  uint32_t hi;
+                  split_pack2(acc[i], acc[i + 1], hi, r[m]);
+                } else {
+                  r[m] = pack2_hi(acc[i], acc[i + 1]);
+                }
+              }
+              // this lane addresses row (lane & 7) of matrix lane >> 3: pixel 8 (jj + lane / 16) + lane % 8 of the half
+              const int p = 8 * (jj + (lane >> 4)) + (lane & 7), ch = 2 * (warp & 3) + ((lane >> 3) & 1);
+              stmatrix_x4_trans(stg_u + p * 128 + ((ch ^ (p & 7)) << 4), r[0], r[1], r[2], r[3]);
+            }
+            wg_sync();
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+              const int idx = 128 * k + t128, p = idx >> 3, ch = idx & 7;
+              const int py = y_wg + 8 * half + (p >> 3), px = x_t + (p & 7);
+              if (live && py < H && px < W) {
+                const uint4 v = *reinterpret_cast<const uint4*>(stg + p * 128 + ((ch ^ (p & 7)) << 4));
+                const int64_t opix = ((int64_t)b * out_H + py) * out_W + px;
+                *reinterpret_cast<uint4*>(dst + opix * out_C + out_c_off + 8 * ch) = v;
+              }
+            }
+          }
+        }
+        continue;
+      }
       auto value = [&](int h, int j, int e) {
         const int i = 4 * j + 2 * h + e;
         return (kFused && !kOne) ? acc[i] + acc[(i + BN / 2) % kAccRegs] : acc[i];
@@ -558,7 +663,7 @@ int smem_bytes_for(const ConvProblem& h, int bn) {
   const int planes = h.passes == 1 ? 1 : 2;
   const int w = h.v2_resident ? nkb * w_tap_bytes(bn, h.kchunk, planes) : h.v2_nw * w_tap_bytes(bn, h.kchunk, planes);
   return h.v2_na * a_stage_bytes_h(h.kchunk, h.tile_h, h.tile_w, h.halo, planes) + w + kFixedBytes +
-         (h.epi_mode == 3 ? kHeadBytes : 0);
+         epi_scratch_bytes(h.epi_mode, h.pxn);
 }
 
 }  // namespace
@@ -570,11 +675,11 @@ namespace {
 // the wgmma group AFTER the one that read it has been committed, and that group reads the next stage of the same
 // ring: both rings therefore need at least two slots, or producer and consumers wait on each other forever.
 // Returns false when the shape cannot get them within the shared-memory budget.
-bool ring_depths(int kc, int tile_h, int tile_w, int halo, int planes, int bn, int cout, int ktot, int epi_mode,
+bool ring_depths(int kc, int tile_h, int tile_w, int halo, int planes, int bn, int cout, int ktot, int epi_mode, int pxn,
                  int& resident, int& na, int& nw) {
   const int wtap = w_tap_bytes(bn, kc, planes);
   const int w_all = (ktot / kc) * wtap;
-  const int kLimit = kSmemLimit - (epi_mode == 3 ? kHeadBytes : 0);   // flow-head epilogue scratch
+  const int kLimit = kSmemLimit - epi_scratch_bytes(epi_mode, pxn);   // flow-head / pixels-on-N store scratch
   const int kAStage = a_stage_bytes_h(kc, tile_h, tile_w, halo, planes);
   if (cout <= bn && w_all + 2 * kAStage + kFixedBytes <= kLimit) {
     resident = 1;
@@ -609,7 +714,7 @@ void conv3x3_tc_pick_tile(int H, int W, int B, int cout, int kc, int passes, int
   tile_w = 8;
   for (auto& c : cand) {
     int res, na, nw;
-    if (!ring_depths(kc, c[0], c[1], 0, passes == 1 ? 1 : 2, bn, cout, ktot, epi_mode, res, na, nw)) continue;
+    if (!ring_depths(kc, c[0], c[1], 0, passes == 1 ? 1 : 2, bn, cout, ktot, epi_mode, 0, res, na, nw)) continue;
     const long tiles = (long)B * ((H + c[0] - 1) / c[0]) * ((W + c[1] - 1) / c[1]) * n_nt;
     const long waves = (tiles + num_sms - 1) / num_sms;
     const double cost = (double)waves * (c[0] + 2.0) / c[0] * (1.0 + 1e-3 * (c[1] / 8));
@@ -628,18 +733,19 @@ bool conv3x3_tc_plan(ConvProblem& h, int num_sms) {
   const int wtap = w_tap_bytes(bn, h.kchunk, planes);
   const int w_all = (h.ktot / h.kchunk) * wtap;
   const bool can_resident = h.cout <= bn;
-  const int kLimit = kSmemLimit - (h.epi_mode == 3 ? kHeadBytes : 0);
-  // wide halo (the engine allows it per chunk size): 16x8 tiles only; resident weights win when both do not fit
-  if (h.halo && (h.tile_h != 16 || h.tile_w != 8 ||
+  const int kLimit = kSmemLimit - epi_scratch_bytes(h.epi_mode, h.pxn);
+  // wide halo (the engine allows it per chunk size): 16x8 (pixels on N: 32x8) tiles only; resident weights win when
+  // both do not fit
+  if (h.halo && (h.tile_h != (h.pxn ? 32 : 16) || h.tile_w != 8 ||
                  (can_resident && w_all + 2 * a_stage_bytes_h(h.kchunk, h.tile_h, h.tile_w, 0, planes) + kFixedBytes <= kLimit &&
                   w_all + 2 * a_stage_bytes_h(h.kchunk, h.tile_h, h.tile_w, 1, planes) + kFixedBytes > kLimit)))
     h.halo = 0;
-  bool ok = ring_depths(h.kchunk, h.tile_h, h.tile_w, h.halo, planes, bn, h.cout, h.ktot, h.epi_mode, h.v2_resident,
-                        h.v2_na, h.v2_nw);
+  bool ok = ring_depths(h.kchunk, h.tile_h, h.tile_w, h.halo, planes, bn, h.cout, h.ktot, h.epi_mode, h.pxn,
+                        h.v2_resident, h.v2_na, h.v2_nw);
   if (!ok && h.halo) {
     h.halo = 0;
-    ok = ring_depths(h.kchunk, h.tile_h, h.tile_w, 0, planes, bn, h.cout, h.ktot, h.epi_mode, h.v2_resident, h.v2_na,
-                     h.v2_nw);
+    ok = ring_depths(h.kchunk, h.tile_h, h.tile_w, 0, planes, bn, h.cout, h.ktot, h.epi_mode, h.pxn, h.v2_resident,
+                     h.v2_na, h.v2_nw);
   }
   const int nsp = h.B * h.tiles_y * h.tiles_x, n_nt = (h.cout + bn - 1) / bn;
   if (h.pair) {   // (2,1,1) clusters, one work item = a pair of spatial tiles
@@ -651,18 +757,18 @@ bool conv3x3_tc_plan(ConvProblem& h, int num_sms) {
   return ok;
 }
 
-template <int BN, int KC>
+template <int BN, int KC, bool kPxN = false>
 struct Variants {
-  // every (kPartial, kHalo, kOne, kRes) instantiation of one (BN, KC) kernel, indexed by the four bits
+  // every (kPartial, kHalo, kOne, kRes) instantiation of one (BN, KC, kPxN) kernel, indexed by the four bits
   static constexpr void (*kFn[16])(const ConvProblem*) = {
-      k_conv3x3_tc<BN, KC, false, false, false, false>, k_conv3x3_tc<BN, KC, false, false, false, true>,
-      k_conv3x3_tc<BN, KC, false, false, true, false>,  k_conv3x3_tc<BN, KC, false, false, true, true>,
-      k_conv3x3_tc<BN, KC, false, true, false, false>,  k_conv3x3_tc<BN, KC, false, true, false, true>,
-      k_conv3x3_tc<BN, KC, false, true, true, false>,   k_conv3x3_tc<BN, KC, false, true, true, true>,
-      k_conv3x3_tc<BN, KC, true, false, false, false>,  k_conv3x3_tc<BN, KC, true, false, false, true>,
-      k_conv3x3_tc<BN, KC, true, false, true, false>,   k_conv3x3_tc<BN, KC, true, false, true, true>,
-      k_conv3x3_tc<BN, KC, true, true, false, false>,   k_conv3x3_tc<BN, KC, true, true, false, true>,
-      k_conv3x3_tc<BN, KC, true, true, true, false>,    k_conv3x3_tc<BN, KC, true, true, true, true>};
+      k_conv3x3_tc<BN, KC, false, false, false, false, kPxN>, k_conv3x3_tc<BN, KC, false, false, false, true, kPxN>,
+      k_conv3x3_tc<BN, KC, false, false, true, false, kPxN>,  k_conv3x3_tc<BN, KC, false, false, true, true, kPxN>,
+      k_conv3x3_tc<BN, KC, false, true, false, false, kPxN>,  k_conv3x3_tc<BN, KC, false, true, false, true, kPxN>,
+      k_conv3x3_tc<BN, KC, false, true, true, false, kPxN>,   k_conv3x3_tc<BN, KC, false, true, true, true, kPxN>,
+      k_conv3x3_tc<BN, KC, true, false, false, false, kPxN>,  k_conv3x3_tc<BN, KC, true, false, false, true, kPxN>,
+      k_conv3x3_tc<BN, KC, true, false, true, false, kPxN>,   k_conv3x3_tc<BN, KC, true, false, true, true, kPxN>,
+      k_conv3x3_tc<BN, KC, true, true, false, false, kPxN>,   k_conv3x3_tc<BN, KC, true, true, false, true, kPxN>,
+      k_conv3x3_tc<BN, KC, true, true, true, false, kPxN>,    k_conv3x3_tc<BN, KC, true, true, true, true, kPxN>};
   static cudaError_t configure() {
     for (auto fn : kFn) {
       const cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
@@ -672,6 +778,7 @@ struct Variants {
   }
   static cudaError_t launch(const ConvProblem* d_prob, const ConvProblem& h, cudaStream_t st) {
     if (h.v2_na < 2 || (!h.v2_resident && h.v2_nw < 2)) return cudaErrorInvalidValue;   // see ring_depths
+    if (kPxN && (h.pair || h.tile_h != 32 || h.tile_w != 8 || h.epi_mode != 0)) return cudaErrorInvalidValue;
     const bool partial = h.v2_part_hi > h.v2_part_lo;
     const int idx = (partial ? 8 : 0) | (h.halo ? 4 : 0) | (h.passes == 1 ? 2 : 0) | (h.v2_resident && h.straight ? 1 : 0);
     if (!h.pair) {
@@ -701,6 +808,8 @@ cudaError_t conv3x3_tc_configure() {
   if (e != cudaSuccess) return e;
   FILM_CFG(32, 64) FILM_CFG(64, 64) FILM_CFG(128, 64) FILM_CFG(256, 64) FILM_CFG(32, 32) FILM_CFG(64, 32)
 #undef FILM_CFG
+  e = Variants<64, 64, true>::configure();
+  if (e != cudaSuccess) return e;
   return cudaSuccess;
 }
 
@@ -714,7 +823,7 @@ cudaError_t launch_conv3x3_tc(const ConvProblem* d_prob, const ConvProblem& h, c
   switch (bn) {
     case 256: return Variants<256, 64>::launch(d_prob, h, st);
     case 128: return Variants<128, 64>::launch(d_prob, h, st);
-    case 64: return Variants<64, 64>::launch(d_prob, h, st);
+    case 64: return h.pxn ? Variants<64, 64, true>::launch(d_prob, h, st) : Variants<64, 64>::launch(d_prob, h, st);
     default: return Variants<32, 64>::launch(d_prob, h, st);
   }
 }

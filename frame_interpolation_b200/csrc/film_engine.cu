@@ -469,6 +469,7 @@ struct Plan {
   int fuse_flow_head = 1;     // flow head (conv_3, conv_4, residual add) in conv_2 epilogue: 1 = level 0, 2 = levels 0 and 1
   int plane_skip = 1;         // lo planes that no consumer reads are neither gathered nor written
   int mma_straight = 1;       // straight-line MMA issue for resident weights
+  int conv3x3_pxn = 1;        // pixels on N for the 64 -> 64 persistent layers: 0 off, 1 where 32x8 tiles give 2 waves, 2 always
   std::vector<void*> allocs;
   int64_t arena_bytes = 0;
   std::vector<ConvProblem> h_probs;
@@ -482,6 +483,7 @@ struct Plan {
     int lane;                  // stream lane the op is enqueued on
     std::vector<int> waits;    // tokens (events) the op waits for before it starts
     std::vector<int> signals;  // tokens recorded after the op
+    std::string form = "";     // conv kernel form: "3x3", "3x3_pxn" (persistent kernel), "tc" (generic), "simt"
   };
   std::vector<Op> ops;
   std::vector<float> op_ms;  // filled by timed eager runs
@@ -599,9 +601,24 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   const bool v2 = P.conv3x3_v2 && P.conv_impl == 0 && pc.ntaps == 9 && (out || epi_mode >= 2) && sy == 1 && sx == 1 &&
                   (kc == kChunk || pc.cout <= 64);
   cp.epi_mode = epi_mode;
+  // pixels on the wgmma N dimension (film_conv3x3_tc.cu): the Cout = 64 layers with 64-channel chunks and a plain or
+  // pooled store run on 32x8 tiles.  By default only where those still give two waves over the SMs, and not with a
+  // source that skips k-steps: fusion_conv1@L0 measured slower on the new form (4.26 -> 4.52 ms, H100 SXM, 400 W);
+  // its side-source stages issue one k-step per 16 KiB weight tap, and with 256-pixel tiles its streamed weight ring
+  // has only two slots
+  const long pxn_tiles = (long)cp.B * ((cp.H + 31) / 32) * ((cp.W + 7) / 8);
+  bool skips_ksteps = false;
+  for (size_t s = 0; s < pc.src_chunks.size(); ++s)
+    if (pc.src_chunks[s] > 0 && pc.src_ksteps[s] != kc / 16) skips_ksteps = true;
+  cp.pxn = (v2 && P.conv3x3_pxn && pc.cout == 64 && kc == kChunk && epi_mode == 0 && out && out_c_off % 8 == 0 &&
+            out->C % 8 == 0 && (!pool_out || pool_out->C % 8 == 0) &&
+            (P.conv3x3_pxn >= 2 || (pxn_tiles >= 2L * P.num_sms && !skips_ksteps))) ? 1 : 0;
   int box_h, box_w;
   if (v2) {
-    if (pool_out) {
+    if (cp.pxn) {
+      cp.tile_h = 32;
+      cp.tile_w = 8;
+    } else if (pool_out) {
       cp.tile_h = 16;  // the fused pool of a 16x8 tile finds each 2x2 partner in lane ^ 4 and the thread's second fragment row
       cp.tile_w = 8;
     } else {
@@ -677,14 +694,14 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   }
   cp.group = 1;
   // wide halo level: 1 = CTA-pair layers, 2 = + every persistent layer (64-channel chunks), 3 = + 32-channel chunks
-  int halo_ok = (v2 && cp.tile_h == 16 && cp.tile_w == 8) ? P.conv3x3_halo : 0;
+  int halo_ok = (v2 && cp.tile_h == (cp.pxn ? 32 : 16) && cp.tile_w == 8) ? P.conv3x3_halo : 0;
   if (kc != kChunk && halo_ok < 3) halo_ok = 0;
   cp.halo = halo_ok >= 2;
   if (v2 && !conv3x3_tc_plan(cp, P.num_sms))
     throw Error{FILM_ERR_UNSUPPORTED, "persistent 3x3 conv: shared-memory rings do not fit (" + tag + ")"};
   // CTA pair ((2,1,1) clusters sharing every streamed weight tap by TMA multicast): layers that stream their weights, on the
   // large levels (conv3x3_2cta = 1) or on every level (2); the RGB / flow-head epilogues stay on single CTAs
-  if (v2 && P.conv3x3_2cta && epi_mode < 2 && !cp.v2_resident &&
+  if (v2 && P.conv3x3_2cta && epi_mode < 2 && !cp.v2_resident && !cp.pxn &&
       (P.conv3x3_2cta >= 2 || (long)cp.B * cp.tiles_y * cp.tiles_x >= 4L * P.num_sms)) {
     cp.pair = 1;
     if (halo_ok >= 1) cp.halo = 1;
@@ -717,7 +734,7 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   double k_issued = 0;  // skipped all-zero k-steps are not issued work
   for (size_t si = 0; si < pc.src_chunks.size(); ++si)
     k_issued += (double)pc.src_chunks[si] * pc.ntaps * (v2 ? pc.src_ksteps[si] * 16 : pc.kchunk);
-  P.mma_flops += (double)cp.passes * 2.0 * (double)cp.B * cp.tiles_y * cp.tiles_x * kTileM * k_issued *
+  P.mma_flops += (double)cp.passes * 2.0 * (double)cp.B * cp.tiles_y * cp.tiles_x * (cp.tile_h * cp.tile_w) * k_issued *
                  (double)(((pc.cout + bn - 1) / bn) * bn);
   // algorithmic HBM bytes of this call site: every source plane it consumes read once, every destination plane written once
   double alg_bytes = 0;
@@ -739,6 +756,7 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
     return v2 ? launch_conv3x3_tc(pp->d_probs + idx, pp->h_probs[idx], st)
               : launch_conv_tc(pp->d_probs + idx, pp->h_probs[idx], st);
   }, 2.0 * ref_macs_per_px * (double)cp.B * cp.H * cp.W, alg_bytes);
+  P.ops.back().form = impl == 1 ? "simt" : !v2 ? "tc" : cp.pxn ? "3x3_pxn" : "3x3";
   return idx;
 }
 
@@ -752,6 +770,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
   P.plane_skip = (fe_conv0_tc & 8) ? 0 : 1;
   P.fuse_flow_head = (fe_conv0_tc & 64) ? 0 : ((fe_conv0_tc & 128) ? 2 : 1);
   P.mma_straight = (fe_conv0_tc & 16) ? 0 : 1;
+  P.conv3x3_pxn = (fe_conv0_tc >> 8) & 3;
   P.onepass_mask = onepass_mask;
   P.reuse = !keep_debug && !use_lanes && !(fe_conv0_tc & 32);
   P.h = h;
@@ -1208,6 +1227,8 @@ struct film_handle {
   int fuse_rgb_head = 1;  // 1 = RGB head + crop in the epilogue of fusion_conv2@L0 (default), 0 = separate kernel
   int plane_skip = 1, mma_straight = 1, arena_reuse = 1;   // optimisations, individually switchable (A/B, bisecting)
   int fuse_flow_head = 1;
+  int conv3x3_pxn = 1;  // pixels on N for the Cout = 64 persistent 3x3 layers: 0 off, 1 where 32x8 tiles give two waves
+                        // over the SMs (default), 2 every eligible layer
   uint8_t* u8_stage = nullptr;  // film_interpolate_u8: [x0][x1][out] on the device
   size_t u8_bytes = 0;
   int num_sms = 132;
@@ -1277,7 +1298,7 @@ static void drop_plans(film_handle* h) {
 static Plan* get_plan(film_handle* h, int hh, int ww, int align) {
   char key[96];
   snprintf(key, sizeof(key), "%dx%d_a%d_i%d_v%d_l%d_p%d_h%d_m%x_d%d", hh, ww, align > 0 ? align : 0, h->conv_impl, h->conv3x3_v2,
-           h->use_lanes, h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->keep_debug * 256 + h->fuse_flow_head * 64 + h->arena_reuse * 32 + h->mma_straight * 16 + h->plane_skip * 8 +
+           h->use_lanes, h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->conv3x3_pxn * 512 + h->keep_debug * 256 + h->fuse_flow_head * 64 + h->arena_reuse * 32 + h->mma_straight * 16 + h->plane_skip * 8 +
                h->fuse_rgb_head * 2 + h->fe_conv0_tc);
   auto it = h->plans.find(key);
   if (it != h->plans.end()) return it->second.get();
@@ -1286,7 +1307,7 @@ static Plan* get_plan(film_handle* h, int hh, int ww, int align) {
     p = build_plan(*h->model, hh, ww, align, h->conv_impl, h->keep_debug != 0, h->conv3x3_v2, h->num_sms,
                    h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->use_lanes != 0, h->fe_conv0_tc | (h->fuse_rgb_head ? 0 : 2) | (h->plane_skip ? 0 : 8) |
                        (h->mma_straight ? 0 : 16) | (h->arena_reuse ? 0 : 32) | (h->fuse_flow_head ? 0 : 64) |
-                       (h->fuse_flow_head >= 2 ? 128 : 0));
+                       (h->fuse_flow_head >= 2 ? 128 : 0) | (h->conv3x3_pxn << 8));
   } catch (const Error& e0) {
     if (e0.code != FILM_ERR_CUDA) throw;  // only an allocation failure is worth a retry
     // Every cached shape keeps its activation arena (GBs at 1080p).  If a new shape does not fit next to
@@ -1296,7 +1317,7 @@ static Plan* get_plan(film_handle* h, int hh, int ww, int align) {
     p = build_plan(*h->model, hh, ww, align, h->conv_impl, h->keep_debug != 0, h->conv3x3_v2, h->num_sms,
                    h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->use_lanes != 0, h->fe_conv0_tc | (h->fuse_rgb_head ? 0 : 2) | (h->plane_skip ? 0 : 8) |
                        (h->mma_straight ? 0 : 16) | (h->arena_reuse ? 0 : 32) | (h->fuse_flow_head ? 0 : 64) |
-                       (h->fuse_flow_head >= 2 ? 128 : 0));
+                       (h->fuse_flow_head >= 2 ? 128 : 0) | (h->conv3x3_pxn << 8));
   }
   if (h->use_graph) {
     cudaGraph_t g = nullptr;
@@ -1454,6 +1475,7 @@ int film_set_option(film_handle* h, const char* name, int value) {
   else if (n == "plane_skip") h->plane_skip = value ? 1 : 0;
   else if (n == "fuse_flow_head") h->fuse_flow_head = value < 0 ? 0 : (value > 2 ? 2 : value);
   else if (n == "mma_straight") h->mma_straight = value ? 1 : 0;
+  else if (n == "conv3x3_pxn") h->conv3x3_pxn = value < 0 ? 0 : (value > 2 ? 2 : value);
   else if (n == "arena_reuse") h->arena_reuse = value ? 1 : 0;
   else if (n == "clear_plans") drop_plans(h);
   else {
@@ -1484,6 +1506,7 @@ int film_get_option(film_handle* h, const char* name, int* value) {
   else if (!strcmp(name, "onepass_default")) *value = (int)kDefaultOnepassMask;
   else if (!strcmp(name, "conv3x3_halo")) *value = h->conv3x3_halo;
   else if (!strcmp(name, "conv3x3_2cta")) *value = h->conv3x3_2cta;
+  else if (!strcmp(name, "conv3x3_pxn")) *value = h->conv3x3_pxn;
   else if (!strcmp(name, "keep_debug")) *value = h->keep_debug;
   else return FILM_ERR_ARG;
   return FILM_OK;
@@ -1906,12 +1929,12 @@ int film_profile(film_handle* h, film_profile_t* out) {
 int film_op_table(film_handle* h, char* buf, int64_t buf_size, int64_t* needed) {
   if (!h || !h->last_plan) return FILM_ERR_ARG;
   try {
-  std::string out = "idx,category,name,ms,ref_flops,alg_bytes\n";
+  std::string out = "idx,category,name,ms,ref_flops,alg_bytes,form\n";
   Plan* P = h->last_plan;
   for (size_t i = 0; i < P->ops.size(); ++i) {
     char line[256];
-    snprintf(line, sizeof(line), "%zu,%d,%s,%.6f,%.0f,%.0f\n", i, P->ops[i].category, P->ops[i].name.c_str(),
-             i < P->op_ms.size() ? P->op_ms[i] : -1.f, P->ops[i].flops, P->ops[i].bytes);
+    snprintf(line, sizeof(line), "%zu,%d,%s,%.6f,%.0f,%.0f,%s\n", i, P->ops[i].category, P->ops[i].name.c_str(),
+             i < P->op_ms.size() ? P->op_ms[i] : -1.f, P->ops[i].flops, P->ops[i].bytes, P->ops[i].form.c_str());
     out += line;
   }
   if (needed) *needed = (int64_t)out.size() + 1;

@@ -191,6 +191,15 @@ __device__ __forceinline__ void acc_fence(float* d) {
   for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
+// Four 8x8 b16 matrices, each given as one register per thread in the accumulator-fragment layout (row lane / 4,
+// columns 2 (lane % 4) + {0, 1}), stored TRANSPOSED: lane l supplies the shared address of row l % 8 of matrix l / 8,
+// and that row receives column l % 8 of the matrix (16 bytes).
+__device__ __forceinline__ void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1),
+               "r"(r2), "r"(r3)
+               : "memory");
+}
+
 // Register reallocation between warpgroups (the producer warpgroup hands its registers to the consumers)
 template <int N>
 __device__ __forceinline__ void regs_dec() {

@@ -301,7 +301,7 @@ class Interpolator:
         for r in rows[1:]:
             v = r.split(",")
             out.append({"idx": int(v[0]), "category": int(v[1]), "name": v[2], "ms": float(v[3]),
-                        "ref_flops": float(v[4]), "alg_bytes": float(v[5])})
+                        "ref_flops": float(v[4]), "alg_bytes": float(v[5]), "form": v[6]})
         return out
 
     @property

@@ -149,6 +149,9 @@ FILM_API int film_profile(film_handle* h, film_profile_t* out);
  *   "conv3x3_halo": wide halo boxes of the persistent kernel -- one (64 ch, 10 px, 18 rows) TMA box per chunk serves all
  *                   nine taps (wgmma descriptors at pixel offsets): 3 = 64- and 32-channel chunks (default),
  *                   2 = 64-channel chunks only, 1 = CTA-pair layers only, 0 = three dx-shifted 8-px boxes
+ *   "conv3x3_pxn" : persistent 3x3 layers with Cout = 64, 64-channel chunks and a plain or pooled store put the pixels
+ *                   on the wgmma N dimension (m64n128k16, weight tap as the M operand, 32x8 tiles): 1 = where 32x8 tiles
+ *                   still give two waves over the SMs and no source skips k-steps (default), 2 = every such layer, 0 = off
  *   "fe_conv0_tc" : cfeat_conv_0 (3 -> 64, K = 27): 0 = register-tiled fp32 FMA kernel reading the fp32 image directly
  *                   (default: exact fp32 arithmetic, no widened image tensor), 1 = tensor-core kernel over a 32-channel-
  *                   padded split image
@@ -171,7 +174,8 @@ FILM_API int film_profile(film_handle* h, film_profile_t* out);
  *                   three-pass split product.  The default is a measured per-stage plan;
  *                   0 = every conv three-pass (fp32-grade).  "onepass_default" (any value) restores it. */
 FILM_API int film_set_option(film_handle* h, const char* name, int value);
-/* Reads back an integer option ("onepass_mask", "onepass_default", "conv3x3_halo", "conv3x3_2cta", "keep_debug"). */
+/* Reads back an integer option ("onepass_mask", "onepass_default", "conv3x3_halo", "conv3x3_2cta", "conv3x3_pxn",
+ * "keep_debug"). */
 FILM_API int film_get_option(film_handle* h, const char* name, int* value);
 
 /* Stages of the precision plan: film_stage_count() names ("fe_i0_k01", "flow_L3", "fus2_c1", ...), index =
@@ -185,8 +189,9 @@ FILM_API int film_stage_name(int stage, char* buf, int buf_size);
 FILM_API int film_debug_read(film_handle* h, const char* name, float* dst, int64_t* count);
 
 /* Per-op table of the plan used by the last call, as CSV text
- * "idx,category,name,ms,ref_flops,alg_bytes" (category 0 = tensor-core conv, 1 = warp gather,
- * 2 = other bandwidth kernels). `ms` is filled by calls made with option "time_ops" = 1
+ * "idx,category,name,ms,ref_flops,alg_bytes,form" (category 0 = tensor-core conv, 1 = warp gather,
+ * 2 = other bandwidth kernels; form = the kernel of a conv: "3x3" / "3x3_pxn" persistent 3x3 kernel, the latter with
+ * pixels on N, "tc" generic wgmma kernel, "simt" validation kernel, empty otherwise). `ms` is filled by calls made with option "time_ops" = 1
  * (eager run, one CUDA event pair per kernel on the launching stream), else -1.
  * *needed receives the buffer size required. */
 FILM_API int film_op_table(film_handle* h, char* buf, int64_t buf_size, int64_t* needed);
