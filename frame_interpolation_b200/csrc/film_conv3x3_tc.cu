@@ -451,12 +451,13 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
         const int y_wg = ty * kTileH + 16 * wg, x_t = tx * kTileW;
         if (do_pool) {
           // 2x2 partners in the thread's own registers: the next column is e ^ 1, the next row is j + 1.  The lane of
-          // the odd cout (lane ^ 4) hands its sum over, and the even-cout lane stores the pair
+          // the odd cout (lane ^ 4) hands its sum over, and the even-cout lane stores the pair.  A pooled pixel is
+          // written only when its whole 2x2 window is inside the frame (VALID pooling floors odd sizes)
           const int px = x_t + 2 * q;
 #pragma unroll
           for (int j = 0; j < 16; j += 2) {
             const int py = y_wg + j;
-            const bool ok = live && py < H && px < W && !(lane & 4);
+            const bool ok = live && (py >> 1) < (out_H >> 1) && (px >> 1) < (out_W >> 1) && !(lane & 4);
             const int64_t ppix = ((int64_t)b * (out_H >> 1) + (py >> 1)) * (out_W >> 1) + (px >> 1);
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
@@ -612,10 +613,12 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
           valid[h] = live && (py < H) && (px < W);
           opix[h] = ((int64_t)b * out_H + py) * out_W + px;
         }
-        // the lane with the even tile column of row r0 owns the pooled pixel (H, W are even; pool implies 16x8 tiles)
+        // the lane with the even tile column of row r0 owns the pooled pixel (pool implies 16x8 tiles).  It is written
+        // only when the whole 2x2 window is inside the frame: VALID pooling floors odd sizes
         const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-        const int64_t ppix = ((int64_t)b * (out_H >> 1) + ((ty * kTileH + r0 / kTileW) >> 1)) * (out_W >> 1) +
-                             ((tx * kTileW + r0 % kTileW) >> 1);
+        const int py0 = ty * kTileH + r0 / kTileW, px0 = tx * kTileW + r0 % kTileW;
+        const bool pool_ok = live && (py0 >> 1) < (out_H >> 1) && (px0 >> 1) < (out_W >> 1) && !(lane & 4);
+        const int64_t ppix = ((int64_t)b * (out_H >> 1) + (py0 >> 1)) * (out_W >> 1) + (px0 >> 1);
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
           const int c = 8 * j + 2 * q;
@@ -645,7 +648,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
               a[h][1] = f1 + __shfl_xor_sync(0xffffffffu, f1, 4);
             }
           }
-          if (do_pool && valid[0] && !(lane & 4)) {
+          if (do_pool && pool_ok) {
             uint32_t hi, lo;
             split_pack2((a[0][0] + a[1][0]) * 0.25f, (a[0][1] + a[1][1]) * 0.25f, hi, lo);
             *reinterpret_cast<uint32_t*>(pool_hi + ppix * pool_C + n0 + c) = hi;

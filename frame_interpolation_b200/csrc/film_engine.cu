@@ -302,6 +302,7 @@ struct Model {
   PackedConv flow_c3[4];                         // predictor p, 1x1 conv_3 (tensor-core, fused head)
   float *flow_w3[4], *flow_b3[4], *flow_w4[4], *flow_b4[4];
   PackedConv fus_up[4][4];                       // level i, parity class py*2+px
+  PackedConv fus_up_2x2[4];                      // level i, plain 2x2 SAME conv on the resized grid (non-2x levels)
   PackedConv fus_c1[4], fus_c2[4];
   float *rgb_w = nullptr, *rgb_b = nullptr;
 
@@ -371,6 +372,10 @@ struct Model {
       for (int py = 0; py < 2; ++py)
         for (int px = 0; px < 2; ++px)
           fus_up[i][py * 2 + px] = pack_conv(k0, b0, up_src, taps_up2x2(py, px), allocs);
+      // the same conv on the fine grid, for levels whose size is not exactly twice the coarser one: the nearest
+      // resize is then a gather of its own, and TMA's out-of-bounds zero fill is the SAME bottom/right padding
+      fus_up_2x2[i] = pack_conv(k0, b0, up_src, {{0, 0, {{0, 0}}}, {0, 1, {{0, 1}}}, {1, 0, {{1, 0}}}, {1, 1, {{1, 1}}}},
+                                allocs);
       const int a_c = 2 * (3 + C) + 4;
       fus_c1[i] = pack_conv(get_tensor(w, pre + "1/kernel", {3, 3, a_c + nf, nf}),
                             get_tensor(w, pre + "1/bias", {nf}),
@@ -760,6 +765,19 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   return idx;
 }
 
+// eval/interpolator.py:30-63: network size and crop offset of an (h, w) frame padded to `align` (<= 0: no padding)
+static void padded_size(int h, int w, int align, int& H, int& W, int& off_y, int& off_x) {
+  int ph = 0, pw = 0;
+  if (align > 0) {
+    ph = (h % align) ? align - h % align : 0;
+    pw = (w % align) ? align - w % align : 0;
+  }
+  H = h + ph;
+  W = w + pw;
+  off_y = ph / 2;
+  off_x = pw / 2;
+}
+
 static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align, int conv_impl, bool keep_debug,
                                         int conv3x3_v2, int num_sms, int conv3x3_2cta, int conv3x3_halo,
                                         uint32_t onepass_mask, bool use_lanes, int fe_conv0_tc) {
@@ -781,20 +799,10 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
   P.conv3x3_halo = conv3x3_halo;
   P.num_sms = num_sms;
   // eval/interpolator.py:30-63
-  int ph = 0, pw = 0;
-  if (align > 0) {
-    ph = (h % align) ? align - h % align : 0;
-    pw = (w % align) ? align - w % align : 0;
-  }
-  P.H = h + ph;
-  P.W = w + pw;
-  P.off_y = ph / 2;
-  P.off_x = pw / 2;
-  // The reference graph accepts any size (VALID pooling floors, flows and fusion resize to the level size);
-  // this engine implements the 64-aligned case only -- the CLI default (--align 64, eval/interpolator_cli.py:103).
-  if (P.H % 64 || P.W % 64)
-    throw Error{FILM_ERR_UNSUPPORTED,
-                "padded frame size must be a multiple of 64 (2^(pyramid_levels-1)) in this engine; use align=64"};
+  padded_size(h, w, align, P.H, P.W, P.off_y, P.off_x);
+  // Any size: level l is H >> l (VALID pooling floors); a decoder level that is not exactly twice the coarser one
+  // gets a nearest resize of its own before fusion_up (the "any_size" option decides, before the plan cache, whether
+  // such sizes are accepted at all)
   int Hs[kLevels], Ws[kLevels];
   for (int l = 0; l < kLevels; ++l) {
     Hs[l] = P.H >> l;
@@ -1079,7 +1087,37 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
       up_src = {{batch_view(wf[i + 1], 0), 0}, {batch_view(wf[i + 1], 1), 0}, {side[i + 1], 0}};
     else
       up_src = {{net, 0}};
-    if (P.conv_impl == 0) {
+    if (hh != 2 * Hs[i + 1] || ww != 2 * Ws[i + 1]) {
+      // fusion.py:133-135 with an odd finer size: the nearest resize has no parity structure, so it runs as a gather
+      // (k_resize_nearest) and conv_0 as a plain 2x2 SAME conv on the fine grid.  The resize's only reader is that
+      // conv: a single-pass one reads hi planes alone, and then its sources' lo planes were not written either
+      const bool hi_only = P.conv_impl == 0 && P.plane_skip && ((P.onepass_mask >> (ST_FUS + 3 * i)) & 1u);
+      std::vector<std::pair<const SplitBuf*, SplitBuf*>> jobs;   // (coarse source, its resized copy)
+      if (i == kFusionLevels - 2) {
+        // both warped batches of the coarsest level in one B = 2 tensor, then the side tensor (its zero padding too:
+        // the generic kernel issues every k-step, and 0 x uninitialised memory could be NaN)
+        jobs.push_back({wf[i + 1], P.split(2, hh, ww, wf[i + 1]->C)});
+        jobs.push_back({side[i + 1], P.split(1, hh, ww, side[i + 1]->C)});
+        up_src = {{batch_view(jobs[0].second, 0), 0}, {batch_view(jobs[0].second, 1), 0}, {jobs[1].second, 0}};
+      } else {
+        jobs.push_back({net, P.split(1, hh, ww, net->C)});
+        up_src = {{jobs[0].second, 0}};
+      }
+      double rbytes = 0;   // every destination channel read once and written once, per plane moved
+      for (auto& j : jobs) rbytes += (double)j.second->pixels() * j.second->C * (hi_only ? 4.0 : 8.0);
+      P.add_op(2, "fusion_resize@L" + std::to_string(i), [jobs, hi_only](cudaStream_t st) {
+        for (auto& j : jobs) {
+          const SplitBuf *s = j.first, *d = j.second;
+          const cudaError_t e = launch_resize_nearest(s->hi, s->lo, s->C, 0, s->B, s->H, s->W, d->hi, d->lo, d->C, 0, d->H,
+                                                      d->W, d->C, hi_only, st);
+          if (e != cudaSuccess) return e;
+        }
+        return cudaSuccess;
+      }, 0, rbytes);
+      add_conv(P, "fusion_up@L" + std::to_string(i), 4.0 * M.fus_up_2x2[i].cin_ref * nf, M.fus_up_2x2[i], up_src, 0, up, 0,
+               ST_FUS + 3 * i, ST_FUS + 3 * i + 1);
+      for (auto& j : jobs) P.release(j.second);   // read by that conv only
+    } else if (P.conv_impl == 0) {
       // the four parity classes share the grid: ONE launch, grid.z = class
       size_t first = 0;
       for (int py = 0; py < 2; ++py)
@@ -1229,6 +1267,7 @@ struct film_handle {
   int fuse_flow_head = 1;
   int conv3x3_pxn = 1;  // pixels on N for the Cout = 64 persistent 3x3 layers: 0 off, 1 where 32x8 tiles give two waves
                         // over the SMs (default), 2 every eligible layer
+  int any_size = 0;     // 1: run padded sizes that are not multiples of 64 (levels with odd sizes), 0: refuse them
   uint8_t* u8_stage = nullptr;  // film_interpolate_u8: [x0][x1][out] on the device
   size_t u8_bytes = 0;
   int num_sms = 132;
@@ -1296,6 +1335,15 @@ static void drop_plans(film_handle* h) {
 }
 
 static Plan* get_plan(film_handle* h, int hh, int ww, int align) {
+  // Checked before the cache lookup: a plan built while "any_size" was 1 must not keep serving its size after the
+  // option is set back to 0.  The plan itself does not depend on the option.
+  if (!h->any_size) {
+    int H, W, oy, ox;
+    padded_size(hh, ww, align, H, W, oy, ox);
+    if (H % 64 || W % 64)
+      throw Error{FILM_ERR_UNSUPPORTED,
+                  "padded frame size must be a multiple of 64 (2^(pyramid_levels-1)) in this engine; use align=64"};
+  }
   char key[96];
   snprintf(key, sizeof(key), "%dx%d_a%d_i%d_v%d_l%d_p%d_h%d_m%x_d%d", hh, ww, align > 0 ? align : 0, h->conv_impl, h->conv3x3_v2,
            h->use_lanes, h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->conv3x3_pxn * 512 + h->keep_debug * 256 + h->fuse_flow_head * 64 + h->arena_reuse * 32 + h->mma_straight * 16 + h->plane_skip * 8 +
@@ -1477,6 +1525,7 @@ int film_set_option(film_handle* h, const char* name, int value) {
   else if (n == "mma_straight") h->mma_straight = value ? 1 : 0;
   else if (n == "conv3x3_pxn") h->conv3x3_pxn = value < 0 ? 0 : (value > 2 ? 2 : value);
   else if (n == "arena_reuse") h->arena_reuse = value ? 1 : 0;
+  else if (n == "any_size") h->any_size = value ? 1 : 0;
   else if (n == "clear_plans") drop_plans(h);
   else {
     h->err = "unknown option " + n;
@@ -1508,6 +1557,7 @@ int film_get_option(film_handle* h, const char* name, int* value) {
   else if (!strcmp(name, "conv3x3_2cta")) *value = h->conv3x3_2cta;
   else if (!strcmp(name, "conv3x3_pxn")) *value = h->conv3x3_pxn;
   else if (!strcmp(name, "keep_debug")) *value = h->keep_debug;
+  else if (!strcmp(name, "any_size")) *value = h->any_size;
   else return FILM_ERR_ARG;
   return FILM_OK;
 }

@@ -598,6 +598,49 @@ cudaError_t launch_fusion_warp(const float* v, const sp_t* feat_hi, const sp_t* 
   return cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------------
+// fusion.py:133 at a level that is not exactly twice the coarser one (odd frame sizes): TF2 NEAREST resize,
+// src = min(floor((dst + 0.5) * in / out), in - 1), in integer arithmetic -- the rule is discontinuous, so a float
+// index could land on the neighbouring source pixel.  One thread per (pixel, 8-channel vector): a raw copy of the
+// split planes, 16 bytes per plane
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ int nearest_src(int dst, int in, int out) {
+  return min((int)(((int64_t)(2 * dst + 1) * in) / (2 * out)), in - 1);
+}
+
+template <bool kHiOnly>
+__global__ void __launch_bounds__(256) k_resize_nearest(const sp_t* __restrict__ src_hi, const sp_t* __restrict__ src_lo,
+                                                        int src_C, int src_c_off, int Hi, int Wi,
+                                                        sp_t* __restrict__ dst_hi, sp_t* __restrict__ dst_lo, int dst_C,
+                                                        int dst_c_off, int Ho, int Wo, int nvec, int64_t n) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int v = (int)(i % nvec);
+  const int64_t p = i / nvec;               // destination pixel over [B][Ho][Wo]
+  const int x = (int)(p % Wo);
+  const int64_t by = p / Wo;
+  const int y = (int)(by % Ho), b = (int)(by / Ho);
+  const int64_t sp = ((int64_t)b * Hi + nearest_src(y, Hi, Ho)) * Wi + nearest_src(x, Wi, Wo);
+  const int64_t so = sp * src_C + src_c_off + 8 * v, d = p * dst_C + dst_c_off + 8 * v;
+  *reinterpret_cast<uint4*>(dst_hi + d) = ldg16(src_hi + so);
+  if constexpr (!kHiOnly) *reinterpret_cast<uint4*>(dst_lo + d) = ldg16(src_lo + so);
+}
+
+cudaError_t launch_resize_nearest(const sp_t* src_hi, const sp_t* src_lo, int src_C, int src_c_off, int B, int Hi, int Wi,
+                                  sp_t* dst_hi, sp_t* dst_lo, int dst_C, int dst_c_off, int Ho, int Wo, int Cn, bool hi_only,
+                                  cudaStream_t st) {
+  if (Cn % 8 || src_C % 8 || dst_C % 8 || src_c_off % 8 || dst_c_off % 8) return cudaErrorInvalidValue;
+  const int nvec = Cn / 8;
+  const int64_t n = (int64_t)B * Ho * Wo * nvec;
+  if (hi_only)
+    k_resize_nearest<true><<<cdiv(n, 256), 256, 0, st>>>(src_hi, src_lo, src_C, src_c_off, Hi, Wi, dst_hi, dst_lo, dst_C,
+                                                          dst_c_off, Ho, Wo, nvec, n);
+  else
+    k_resize_nearest<false><<<cdiv(n, 256), 256, 0, st>>>(src_hi, src_lo, src_C, src_c_off, Hi, Wi, dst_hi, dst_lo, dst_C,
+                                                           dst_c_off, Ho, Wo, nvec, n);
+  return cudaGetLastError();
+}
+
 __global__ void __launch_bounds__(256) k_fusion_side(const float* __restrict__ v,
                                                      const float* __restrict__ img, int H, int W,
                                                      sp_t* __restrict__ side_hi,

@@ -53,6 +53,14 @@ cudaError_t launch_flow_head(const sp_t* x_hi, const sp_t* x_lo, int Cx, int nf,
 // by forward flow; v[0] = forward flow, v[1] = backward flow).
 cudaError_t launch_fusion_warp(const float* v, const sp_t* feat_hi, const sp_t* feat_lo, int H,
                                int W, int C, sp_t* warped_hi, sp_t* warped_lo, bool hi_only, cudaStream_t st);
+// fusion.py:133 when the level is not exactly twice the coarser one: TF2 NEAREST resize of channels
+// [src_c_off, src_c_off + Cn) of a [B][Hi][Wi][src_C] split tensor into channels [dst_c_off, dst_c_off + Cn) of a
+// [B][Ho][Wo][dst_C] one, src = min(floor((dst + 0.5) * in / out), in - 1) per axis (exact integer arithmetic).
+// Channel counts and offsets are multiples of 8.  hi_only: the consumer is a single-pass conv -> only the hi planes
+// are read and written.
+cudaError_t launch_resize_nearest(const sp_t* src_hi, const sp_t* src_lo, int src_C, int src_c_off, int B, int Hi, int Wi,
+                                  sp_t* dst_hi, sp_t* dst_lo, int dst_C, int dst_c_off, int Ho, int Wo, int Cn, bool hi_only,
+                                  cudaStream_t st);
 // side tensor [1][H][W][side_C] split: ch 0-2 warp(img0, .5*bwd), 3-5 warp(img1, .5*fwd),
 // 6-7 .5*bwd, 8-9 .5*fwd, 10-15 zero.
 cudaError_t launch_fusion_side(const float* v, const float* img, int H, int W, sp_t* side_hi,

@@ -82,10 +82,13 @@ def main(argv=None) -> int:
     ap.add_argument("--metrics", default="l1,l2,ssim,psnr")
     ap.add_argument("--output_frames", action="store_true")
     ap.add_argument("--align", type=int, default=64)
+    ap.add_argument("--any_size", action="store_true", help="accept padded sizes that are not multiples of 64")
     ap.add_argument("--device", type=int, default=0)
     a = ap.parse_args(argv)
     from .interpolator import Interpolator
     interp = Interpolator(a.model_path, align=a.align, device=a.device)
+    if a.any_size:
+        interp.set_option("any_size", 1)
     trip = find_triplets(a.triplets)
     if not trip:
         print(f"[film_b200] no triplet folders under {a.triplets}", file=sys.stderr)

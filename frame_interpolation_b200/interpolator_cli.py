@@ -37,6 +37,9 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--align", type=int, default=64)
     p.add_argument("--block_height", type=int, default=1)
     p.add_argument("--block_width", type=int, default=1)
+    p.add_argument("--any_size", action="store_true",
+                   help="Accept padded frame sizes that are not multiples of 64 (e.g. --align 0 at 1920x1080), like the "
+                        "reference graph; off by default.")
     p.add_argument("--output_video", action="store_true")
     p.add_argument("--device", type=int, default=None, help="CUDA device ordinal (default: LOCAL_RANK or 0)")
     return p
@@ -105,6 +108,8 @@ def main(argv=None) -> int:
     directories = sorted(d for d in glob.glob(args.pattern) if os.path.isdir(d))
     mine = directories[rank::world]            # directories are independent: shard them over ranks
     interpolator = Interpolator(args.model_path, args.align, [args.block_height, args.block_width], device=device)
+    if args.any_size:
+        interpolator.set_option("any_size", 1)
     for d in mine:
         n = process_directory(d, interpolator, args.times_to_interpolate, args.fps, args.output_video)
         print(f"[film_b200] {d}: wrote {n} frames to {d}/interpolated_frames", flush=True)

@@ -85,7 +85,8 @@ FILM_API int film_create(film_handle** out, const char* weights_path, int device
 FILM_API void film_destroy(film_handle* h);
 
 /* Host pointers. x0/x1/out: B*H*W*3 floats. align <= 0 disables padding
- * (eval/interpolator.py:149: `align or None`); then H and W must be multiples of 64.
+ * (eval/interpolator.py:149: `align or None`); then H and W must be multiples of 64 unless the
+ * option "any_size" is 1.
  * Blocks until `out` is written. */
 FILM_API int film_interpolate(film_handle* h, const float* x0, const float* x1, const float* dt,
                      int B, int H, int W, int align, float* out);
@@ -164,6 +165,11 @@ FILM_API int film_profile(film_handle* h, film_profile_t* out);
  *                   conv_2 (default), 2 = also on level 1 (64 filters: measured epilogue-bound, slower), 0 = separate launch
  *   "fuse_rgb_head": 1 = the linear 1x1 RGB head and the crop run in the epilogue of the decoder's last 3x3 conv (default;
  *                   the 64-channel activation is never stored), 0 = separate kernel
+ *   "any_size"    : 0 = the padded frame size must be a multiple of 64, anything else fails with status 4 (default),
+ *                   1 = any padded size whose level-5 grid is at least 2x2 runs the reference graph (smaller frames
+ *                   fail with status 1): pyramid levels floor like its VALID pooling, and a decoder level that is not
+ *                   exactly twice the coarser one gets a nearest resize of its own before fusion conv_0.  Only decides
+ *                   whether a size is accepted: a 64-aligned size runs the same plan either way
  *   "use_lanes"   : 1 = enqueue independent branches on separate streams (default 0)
  *   "clear_plans" : (any value) drop every cached (H, W, align) plan -- CUDA graph and activation arena --
  *                   after draining the handle's stream.  Plans are cached per shape and never evicted
@@ -175,7 +181,7 @@ FILM_API int film_profile(film_handle* h, film_profile_t* out);
  *                   0 = every conv three-pass (fp32-grade).  "onepass_default" (any value) restores it. */
 FILM_API int film_set_option(film_handle* h, const char* name, int value);
 /* Reads back an integer option ("onepass_mask", "onepass_default", "conv3x3_halo", "conv3x3_2cta", "conv3x3_pxn",
- * "keep_debug"). */
+ * "keep_debug", "any_size"). */
 FILM_API int film_get_option(film_handle* h, const char* name, int* value);
 
 /* Stages of the precision plan: film_stage_count() names ("fe_i0_k01", "flow_L3", "fus2_c1", ...), index =
