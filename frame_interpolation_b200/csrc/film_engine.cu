@@ -72,6 +72,71 @@ static int fe_stage(int image_level, int conv_k) {
 constexpr uint32_t kDefaultOnepassMask =
     (1u << ST_FE_I0_K23) | (1u << ST_FE_I0_K45) | (1u << ST_FE_I0_K67) |
     (0x1Fu << ST_FLOW_L0) | (0x3Fu << (ST_FUS + 6));
+
+// ----------------------------------------------------------------------------------------
+// engine options (film_set_option): a handle holds one set, each plan a copy of the set it was built from
+// ----------------------------------------------------------------------------------------
+struct Options {
+  int conv_impl = 0;     // 0 = tensor-core kernels, 1 = fp32 CUDA-core validation kernels
+  int use_graph = 1;     // capture each plan's schedule in a CUDA graph
+  int keep_debug = 0;    // keep every intermediate readable (no arena reuse, no fused RGB head)
+  int time_ops = 0;      // eager runs with one CUDA-event pair per op (film_op_table)
+  int use_lanes = 0;     // stream lanes: measured no gain at 1080p (smem-saturating kernels cannot co-reside)
+  int conv3x3_v2 = 1;    // persistent tap-reuse kernel for 3x3 convs
+  int conv3x3_2cta = 0;  // CTA-pair clusters for the streamed-weight 3x3 convs of the large levels: off by default, 1080p
+                         // step 60.5 ms with them against 53.4 ms without (H100 SXM, 400 W; the paired layers run slower)
+  int conv3x3_halo = 3;  // wide halo boxes (one 10-px box per chunk serves nine taps): 0 off, 1 the CTA-pair layers, 2 every
+                         // 64-channel-chunk layer of the persistent kernel, 3 also its 32-channel-chunk layers
+  int conv3x3_pxn = 1;   // pixels on N for the Cout = 64 persistent 3x3 layers: 0 off, 1 where 32x8 tiles give two waves
+                         // over the SMs (default), 2 every eligible layer
+  int onepass_mask = (int)kDefaultOnepassMask;  // precision plan: stages on the single-pass product (see `enum Stage`)
+  int fe_conv0_tc = 0;   // cfeat_conv_0: 0 = fp32 FMA kernel straight from the fp32 image (exact fp32, no widened image
+                         // tensor; K = 27 is not tensor-core work), 1 = tensor-core kernel over the 32-channel-padded image
+  int fuse_rgb_head = 1;   // RGB head + crop in the epilogue of the decoder's last conv, 0 = separate kernel
+  int fuse_flow_head = 1;  // flow head (conv_3, conv_4, residual add) in the conv_2 epilogue: 1 = level 0, 2 = levels 0 and 1
+  int plane_skip = 1;    // lo planes that no consumer reads are neither gathered nor written
+  int mma_straight = 1;  // straight-line MMA issue for resident weights
+  int arena_reuse = 1;   // activation buffers are recycled inside a plan by liveness
+  int any_size = 0;      // 1: run padded sizes that are not multiples of 64 (levels with odd sizes), 0: refuse them
+};
+
+static int as_given(int v) { return v; }
+static int as_bool(int v) { return v ? 1 : 0; }
+static int clamp_0_2(int v) { return v < 0 ? 0 : (v > 2 ? 2 : v); }
+static int stage_bits(int v) { return (int)((uint32_t)v & ((1u << ST_COUNT) - 1u)); }
+struct OptionRow {
+  const char* name;
+  int Options::*field;
+  int (*normalise)(int);  // applied to every value stored, from film_set_option or the environment
+  const char* env;        // environment variable that overrides the default in film_create (nullptr: none)
+  bool plan_key;          // the option shapes the plan: a plan is cached per value
+};
+static const OptionRow kOptions[] = {
+    {"conv_impl", &Options::conv_impl, as_given, nullptr, true},
+    {"use_graph", &Options::use_graph, as_given, nullptr, false},
+    {"keep_debug", &Options::keep_debug, as_given, nullptr, true},
+    {"time_ops", &Options::time_ops, as_given, nullptr, false},
+    {"use_lanes", &Options::use_lanes, as_given, nullptr, true},
+    {"conv3x3_v2", &Options::conv3x3_v2, as_given, nullptr, true},
+    {"conv3x3_2cta", &Options::conv3x3_2cta, as_given, "FILM_2CTA", true},
+    {"conv3x3_halo", &Options::conv3x3_halo, as_given, "FILM_HALO", true},
+    {"conv3x3_pxn", &Options::conv3x3_pxn, clamp_0_2, nullptr, true},
+    {"onepass_mask", &Options::onepass_mask, stage_bits, "FILM_ONEPASS", true},
+    {"fe_conv0_tc", &Options::fe_conv0_tc, as_bool, "FILM_FE0_TC", true},
+    {"fuse_rgb_head", &Options::fuse_rgb_head, as_bool, "FILM_RGB_FUSE", true},
+    {"fuse_flow_head", &Options::fuse_flow_head, clamp_0_2, "FILM_FLOW_HEAD_FUSE", true},
+    {"plane_skip", &Options::plane_skip, as_bool, "FILM_PLANE_SKIP", true},
+    {"mma_straight", &Options::mma_straight, as_bool, "FILM_STRAIGHT", true},
+    {"arena_reuse", &Options::arena_reuse, as_bool, "FILM_ARENA_REUSE", true},
+    // only decides whether a size is accepted (get_plan, before the cache lookup): a 64-aligned size runs the same plan
+    {"any_size", &Options::any_size, as_bool, nullptr, false},
+};
+static const OptionRow& option_row(const char* name) {
+  for (const OptionRow& r : kOptions)
+    if (!strcmp(r.name, name)) return r;
+  throw Error{FILM_ERR_ARG, std::string("unknown option ") + name};
+}
+
 #define FILM_CUDA(expr)                                                                       \
   do {                                                                                        \
     cudaError_t e__ = (expr);                                                                 \
@@ -465,16 +530,12 @@ struct DebugTensor {
 
 struct Plan {
   int h, w, H, W, off_y, off_x;
-  int conv_impl;
-  int conv3x3_v2 = 1, num_sms = 132, conv3x3_2cta = 0;
-  int conv3x3_halo = 0;  // 1: CTA-pair layers, 2: + every persistent layer (64-channel chunks), 3: + 32-channel chunks
-  uint32_t onepass_mask = 0;  // precision plan: stages on the single-pass product
-  int fe_conv0_tc = 0;        // 1: cfeat_conv_0 on the tensor cores (32-channel-padded image), 0: fp32 FMA kernel
-  int fuse_rgb_head = 1;      // RGB head + crop in the epilogue of the decoder's last conv
-  int fuse_flow_head = 1;     // flow head (conv_3, conv_4, residual add) in conv_2 epilogue: 1 = level 0, 2 = levels 0 and 1
-  int plane_skip = 1;         // lo planes that no consumer reads are neither gathered nor written
-  int mma_straight = 1;       // straight-line MMA issue for resident weights
-  int conv3x3_pxn = 1;        // pixels on N for the 64 -> 64 persistent layers: 0 off, 1 where 32x8 tiles give 2 waves, 2 always
+  Options opt;
+  int num_sms = 132;
+  // the conv of precision-plan stage `stage` runs the single-pass product (ST_NONE: not a conv stage)
+  bool onepass(int stage) const { return stage >= 0 && opt.conv_impl == 0 && (((uint32_t)opt.onepass_mask >> stage) & 1u); }
+  // a tensor whose only reader is the single-pass conv of stage `consumer` needs no lo plane: it is not written
+  bool hi_only(int consumer) const { return opt.plane_skip && onepass(consumer); }
   std::vector<void*> allocs;
   int64_t arena_bytes = 0;
   std::vector<ConvProblem> h_probs;
@@ -589,11 +650,12 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
                        const SplitBuf* pool_out = nullptr, bool no_op = false, int epi_mode = 0) {
   // `stage`: precision-plan stage of this conv.  `consumer`: stage of the ONLY reader of the destination when that
   // reader is a conv (ST_NONE otherwise): a single-pass reader never touches the lo plane, so it is not written.
+  const Options& o = P.opt;
   ConvProblem cp;
   memset(&cp, 0, sizeof(cp));
-  cp.passes = (stage >= 0 && P.conv_impl == 0 && ((P.onepass_mask >> stage) & 1u)) ? 1 : 3;
-  cp.out_lo_skip = (consumer >= 0 && P.conv_impl == 0 && !pool_out && P.plane_skip && ((P.onepass_mask >> consumer) & 1u)) ? 1 : 0;
-  cp.straight = P.mma_straight;
+  cp.passes = P.onepass(stage) ? 1 : 3;
+  cp.out_lo_skip = (!pool_out && P.hi_only(consumer)) ? 1 : 0;
+  cp.straight = o.mma_straight;
   const SplitBuf* s0 = sources[0].buf;
   cp.nsrc = (int)sources.size();
   if (cp.nsrc != (int)pc.src_chunks.size()) throw Error{FILM_ERR_WEIGHTS, "source count mismatch"};
@@ -603,7 +665,7 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   // 3x3 SAME convs with a unit-stride destination run on the persistent tap-reuse kernel
   const int kc = pc.kchunk;
   cp.kchunk = kc;
-  const bool v2 = P.conv3x3_v2 && P.conv_impl == 0 && pc.ntaps == 9 && (out || epi_mode >= 2) && sy == 1 && sx == 1 &&
+  const bool v2 = o.conv3x3_v2 && o.conv_impl == 0 && pc.ntaps == 9 && (out || epi_mode >= 2) && sy == 1 && sx == 1 &&
                   (kc == kChunk || pc.cout <= 64);
   cp.epi_mode = epi_mode;
   // pixels on the wgmma N dimension (film_conv3x3_tc.cu): the Cout = 64 layers with 64-channel chunks and a plain or
@@ -615,9 +677,9 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   bool skips_ksteps = false;
   for (size_t s = 0; s < pc.src_chunks.size(); ++s)
     if (pc.src_chunks[s] > 0 && pc.src_ksteps[s] != kc / 16) skips_ksteps = true;
-  cp.pxn = (v2 && P.conv3x3_pxn && pc.cout == 64 && kc == kChunk && epi_mode == 0 && out && out_c_off % 8 == 0 &&
+  cp.pxn = (v2 && o.conv3x3_pxn && pc.cout == 64 && kc == kChunk && epi_mode == 0 && out && out_c_off % 8 == 0 &&
             out->C % 8 == 0 && (!pool_out || pool_out->C % 8 == 0) &&
-            (P.conv3x3_pxn >= 2 || (pxn_tiles >= 2L * P.num_sms && !skips_ksteps))) ? 1 : 0;
+            (o.conv3x3_pxn >= 2 || (pxn_tiles >= 2L * P.num_sms && !skips_ksteps))) ? 1 : 0;
   int box_h, box_w;
   if (v2) {
     if (cp.pxn) {
@@ -699,15 +761,15 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   }
   cp.group = 1;
   // wide halo level: 1 = CTA-pair layers, 2 = + every persistent layer (64-channel chunks), 3 = + 32-channel chunks
-  int halo_ok = (v2 && cp.tile_h == (cp.pxn ? 32 : 16) && cp.tile_w == 8) ? P.conv3x3_halo : 0;
+  int halo_ok = (v2 && cp.tile_h == (cp.pxn ? 32 : 16) && cp.tile_w == 8) ? o.conv3x3_halo : 0;
   if (kc != kChunk && halo_ok < 3) halo_ok = 0;
   cp.halo = halo_ok >= 2;
   if (v2 && !conv3x3_tc_plan(cp, P.num_sms))
     throw Error{FILM_ERR_UNSUPPORTED, "persistent 3x3 conv: shared-memory rings do not fit (" + tag + ")"};
   // CTA pair ((2,1,1) clusters sharing every streamed weight tap by TMA multicast): layers that stream their weights, on the
   // large levels (conv3x3_2cta = 1) or on every level (2); the RGB / flow-head epilogues stay on single CTAs
-  if (v2 && P.conv3x3_2cta && epi_mode < 2 && !cp.v2_resident && !cp.pxn &&
-      (P.conv3x3_2cta >= 2 || (long)cp.B * cp.tiles_y * cp.tiles_x >= 4L * P.num_sms)) {
+  if (v2 && o.conv3x3_2cta && epi_mode < 2 && !cp.v2_resident && !cp.pxn &&
+      (o.conv3x3_2cta >= 2 || (long)cp.B * cp.tiles_y * cp.tiles_x >= 4L * P.num_sms)) {
     cp.pair = 1;
     if (halo_ok >= 1) cp.halo = 1;
     if (!conv3x3_tc_plan(cp, P.num_sms))
@@ -755,7 +817,7 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   P.last_conv_bytes = alg_bytes;
   if (no_op) return idx;  // the caller launches this problem as part of a group
   Plan* pp = &P;
-  const int impl = P.conv_impl;
+  const int impl = o.conv_impl;
   P.add_op(0, tag, [pp, idx, impl, v2](cudaStream_t st) {
     if (impl == 1) return launch_conv_simt(pp->d_probs + idx, pp->h_probs[idx], st);
     return v2 ? launch_conv3x3_tc(pp->d_probs + idx, pp->h_probs[idx], st)
@@ -778,30 +840,20 @@ static void padded_size(int h, int w, int align, int& H, int& W, int& off_y, int
   off_x = pw / 2;
 }
 
-static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align, int conv_impl, bool keep_debug,
-                                        int conv3x3_v2, int num_sms, int conv3x3_2cta, int conv3x3_halo,
-                                        uint32_t onepass_mask, bool use_lanes, int fe_conv0_tc) {
+static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align, const Options& opt, int num_sms) {
   std::unique_ptr<Plan> pl(new Plan);
   Plan& P = *pl;
-  P.fe_conv0_tc = fe_conv0_tc & 1;
-  P.fuse_rgb_head = (fe_conv0_tc & 2) ? 0 : 1;
-  P.plane_skip = (fe_conv0_tc & 8) ? 0 : 1;
-  P.fuse_flow_head = (fe_conv0_tc & 64) ? 0 : ((fe_conv0_tc & 128) ? 2 : 1);
-  P.mma_straight = (fe_conv0_tc & 16) ? 0 : 1;
-  P.conv3x3_pxn = (fe_conv0_tc >> 8) & 3;
-  P.onepass_mask = onepass_mask;
-  P.reuse = !keep_debug && !use_lanes && !(fe_conv0_tc & 32);
+  P.opt = opt;
+  P.reuse = !opt.keep_debug && !opt.use_lanes && opt.arena_reuse;
+  // the RGB head and the crop run in the epilogue of fusion_conv2@L0 instead of a kernel of their own
+  const bool fuse_rgb = opt.conv_impl == 0 && opt.conv3x3_v2 && opt.fuse_rgb_head && !opt.keep_debug;
   P.h = h;
   P.w = w;
-  P.conv_impl = conv_impl;
-  P.conv3x3_v2 = conv3x3_v2;
-  P.conv3x3_2cta = conv3x3_2cta;
-  P.conv3x3_halo = conv3x3_halo;
   P.num_sms = num_sms;
   // eval/interpolator.py:30-63
   padded_size(h, w, align, P.H, P.W, P.off_y, P.off_x);
   // Any size: level l is H >> l (VALID pooling floors); a decoder level that is not exactly twice the coarser one
-  // gets a nearest resize of its own before fusion_up (the "any_size" option decides, before the plan cache, whether
+  // gets a nearest resize of its own before fusion_up (the option any_size decides, before the plan cache, whether
   // such sizes are accepted at all)
   int Hs[kLevels], Ws[kLevels];
   for (int l = 0; l < kLevels; ++l) {
@@ -826,7 +878,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
   }
   // image pyramid (util.py:38-44): fused into the first conv of each scale when that conv is the FMA kernel (it has the
   // input patch in shared memory anyway); stand-alone pools otherwise (tensor-core first layer, validation path, lanes)
-  const bool fuse_img_pool = P.conv_impl == 0 && !P.fe_conv0_tc && !use_lanes;
+  const bool fuse_img_pool = opt.conv_impl == 0 && !opt.fe_conv0_tc && !opt.use_lanes;
   for (int l = 0; l + 1 < kLevels && !fuse_img_pool; ++l) {
     const float* in = img[l];
     float* out = img[l + 1];
@@ -850,18 +902,18 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
     for (int j = 0; j < depth; ++j) {
       const int r = i + j, c = kFilters << j;
       SplitBuf* t1 = P.split(2, Hs[r], Ws[r], c);
-      if (j == 0 && P.conv_impl == 0 && !P.fe_conv0_tc) {
+      if (j == 0 && opt.conv_impl == 0 && !opt.fe_conv0_tc) {
         // cfeat_conv_0 (K = 27) on the FMA pipes, straight from the fp32 image level (exact fp32 arithmetic)
         const float* im = img[i];
         const int hh = Hs[r], ww = Ws[r];
         const float *w0 = M.conv0_w, *b0 = M.conv0_b;
         sp_t *oh = t1->hi, *ol = t1->lo;
-        const bool lo_skip = P.plane_skip && ((P.onepass_mask >> fe_stage(i, 1)) & 1u);   // only reader: cfeat_conv_1 of this sub-tree
+        const bool lo_skip = P.hi_only(fe_stage(i, 1));   // only reader: cfeat_conv_1 of this sub-tree
         float* pool_dst = (fuse_img_pool && i + 1 < kLevels) ? img[i + 1] : nullptr;   // next pyramid level
         P.add_op(2, std::string(pool_dst ? "fe_conv0+pool@L" : "fe_conv0@L") + std::to_string(r),
                  [=](cudaStream_t st) { return launch_fe_conv0(im, 2, hh, ww, w0, b0, oh, ol, lo_skip, pool_dst, st); },
                  2.0 * 27 * 64 * 2.0 * hh * ww, 2.0 * hh * ww * (3 * 4 + 64 * (lo_skip ? 2.0 : 4.0)));
-      } else if (j == 0 && P.conv_impl == 0 && P.conv3x3_v2) {
+      } else if (j == 0 && opt.conv_impl == 0 && opt.conv3x3_v2) {
         // cfeat_conv_0 on the persistent 3x3 tensor-core kernel: the image is widened to a 32-channel
         // split tensor (3 real channels), K = 9 taps x one 32-channel block
         const float* im = img[i];
@@ -871,7 +923,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
                  [=](cudaStream_t st) { return launch_image_to_split32(im, 2, hh, ww, im32->hi, im32->lo, st); }, 0,
                  2.0 * hh * ww * (12 + 32.0));
         add_conv(P, "fe_conv0@L" + std::to_string(r), 27.0 * 64, M.fe0_3x3, {{im32, 0}}, 1, t1, 0, fe_stage(i, 0), fe_stage(i, 1));
-      } else if (j == 0 && P.conv_impl == 0) {
+      } else if (j == 0 && opt.conv_impl == 0) {
         // generic-kernel variant: im2col-lite (27 -> 32 channels) + a 1x1 conv, K = 32
         const float* im = img[i];
         const int hh = Hs[r], ww = Ws[r];
@@ -896,7 +948,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
       // second conv of the pair writes straight into the cascaded feature tensor slice
       // (replaces the tf.concat at feature_extractor.py:191)
       SplitBuf* pool_target = nullptr;
-      const bool fuse_pool = (j < depth - 1) && P.conv_impl == 0 && P.conv3x3_v2;
+      const bool fuse_pool = (j < depth - 1) && opt.conv_impl == 0 && opt.conv3x3_v2;
       if (j < depth - 1) pool_target = P.split(2, Hs[r + 1], Ws[r + 1], c);
       add_conv(P, "fe_conv" + std::to_string(2 * j + 1) + "@L" + std::to_string(r), 9.0 * c * c, M.fe[2 * j + 1],
                {{t1, 0}}, 1, feat[r], slice_off[j], fe_stage(i, 2 * j + 1), ST_NONE, 1, 1, 0, 0,
@@ -952,7 +1004,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
       const int hc = Hs[l + 1], wc = Ws[l + 1];
       float* vu = vup;
       // the warped features feed flow_conv0 of this level only: a single-pass consumer reads hi planes alone
-      const bool hi_only = P.conv_impl == 0 && P.plane_skip && ((P.onepass_mask >> (ST_FLOW_L0 + l)) & 1u);
+      const bool hi_only = P.hi_only(ST_FLOW_L0 + l);
       const double wbytes = 2.0 * hh * ww * (double)C * (hi_only ? 4.0 : 8.0);
       P.add_op(1, "flow_warp@L" + std::to_string(l), [=](cudaStream_t st) {
         return launch_flow_warp(vprev, hc, wc, f->hi, f->lo, hh, ww, C, vu, warped->hi, warped->lo, hi_only, st);
@@ -985,7 +1037,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
     // level 0 (32-filter predictor): conv_3, conv_4 and the residual add run in conv_2's epilogue.  The kernel supports
     // nf <= 64, but the 64-filter level 1 epilogue (32 x 32 FMAs per pixel) is slower fused than as two launches
     // while level 0 gains -- so by default only level 0 is fused (fuse_flow_head = 2 fuses both).
-    const bool fuse_head = P.conv_impl == 0 && P.conv3x3_v2 && P.fuse_flow_head && nf <= (P.fuse_flow_head >= 2 ? 64 : 32);
+    const bool fuse_head = opt.conv_impl == 0 && opt.conv3x3_v2 && opt.fuse_flow_head && nf <= (opt.fuse_flow_head >= 2 ? 64 : 32);
     if (fuse_head) {
       const size_t ci = add_conv(P, "flow_conv2+head" + lt, 9.0 * nf * nf + 1.0 * nf * (nf / 2) + (nf / 2) * 2.0, M.flow[p][2],
                                  {{c1, 0}}, 1, nullptr, 0, ST_FLOW_L0 + l, ST_NONE, 1, 1, 0, 0, nullptr, false, 3);
@@ -1002,7 +1054,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
       add_conv(P, "flow_conv2" + lt, 9.0 * nf * nf, M.flow[p][2], {{c1, 0}}, 1, c2, 0, ST_FLOW_L0 + l, ST_NONE);
     }
     if (fuse_head) {
-    } else if (P.conv_impl == 1) {
+    } else if (opt.conv_impl == 1) {
       // CUDA-core validation path keeps the standalone fp32 head kernel
       const float *w3 = M.flow_w3[p], *b3 = M.flow_b3[p], *w4 = M.flow_w4[p], *b4 = M.flow_b4[p];
       float *rr = res[l], *vv = v[l];
@@ -1050,7 +1102,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
     const SplitBuf *f = feat[l], *o = wf[l], *sd = side[l];
     // consumers of the warped level: fusion_conv1 of the level (fusion_up of level 3 for the coarsest one)
     const int cons = l == kFusionLevels - 1 ? ST_FUS + 3 * (l - 1) : ST_FUS + 3 * l + 1;
-    const bool hi_only = P.conv_impl == 0 && P.plane_skip && ((P.onepass_mask >> cons) & 1u);
+    const bool hi_only = P.hi_only(cons);
     const double wbytes = 2.0 * hh * ww * (double)C * (hi_only ? 4.0 : 8.0);
     P.add_op(1, "fusion_warp@L" + std::to_string(l), [=](cudaStream_t st) {
       return launch_fusion_warp(vv, f->hi, f->lo, hh, ww, C, o->hi, o->lo, hi_only, st);
@@ -1091,7 +1143,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
       // fusion.py:133-135 with an odd finer size: the nearest resize has no parity structure, so it runs as a gather
       // (k_resize_nearest) and conv_0 as a plain 2x2 SAME conv on the fine grid.  The resize's only reader is that
       // conv: a single-pass one reads hi planes alone, and then its sources' lo planes were not written either
-      const bool hi_only = P.conv_impl == 0 && P.plane_skip && ((P.onepass_mask >> (ST_FUS + 3 * i)) & 1u);
+      const bool hi_only = P.hi_only(ST_FUS + 3 * i);
       std::vector<std::pair<const SplitBuf*, SplitBuf*>> jobs;   // (coarse source, its resized copy)
       if (i == kFusionLevels - 2) {
         // both warped batches of the coarsest level in one B = 2 tensor, then the side tensor (its zero padding too:
@@ -1117,7 +1169,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
       add_conv(P, "fusion_up@L" + std::to_string(i), 4.0 * M.fus_up_2x2[i].cin_ref * nf, M.fus_up_2x2[i], up_src, 0, up, 0,
                ST_FUS + 3 * i, ST_FUS + 3 * i + 1);
       for (auto& j : jobs) P.release(j.second);   // read by that conv only
-    } else if (P.conv_impl == 0) {
+    } else if (opt.conv_impl == 0) {
       // the four parity classes share the grid: ONE launch, grid.z = class
       size_t first = 0;
       for (int py = 0; py < 2; ++py)
@@ -1140,13 +1192,12 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
                    4.0 * M.fus_up[i][0].cin_ref * nf, M.fus_up[i][py * 2 + px], up_src, 0, up, 0, ST_FUS + 3 * i,
                    ST_FUS + 3 * i + 1, 2, 2, py, px);
     }
-    const bool fuse_rgb = (i == 0) && P.conv_impl == 0 && P.conv3x3_v2 && P.fuse_rgb_head && !keep_debug;
     SplitBuf* f1 = P.split(1, hh, ww, cpad);
-    SplitBuf* f2 = fuse_rgb ? nullptr : P.split(1, hh, ww, cpad);
+    SplitBuf* f2 = (fuse_rgb && i == 0) ? nullptr : P.split(1, hh, ww, cpad);
     add_conv(P, "fusion_conv1@L" + std::to_string(i), 9.0 * M.fus_c1[i].cin_ref * nf, M.fus_c1[i],
              {{batch_view(wf[i], 0), 0}, {batch_view(wf[i], 1), 0}, {side[i], 0}, {up, 0}}, 1, f1, 0, ST_FUS + 3 * i + 1,
              ST_FUS + 3 * i + 2);
-    if (fuse_rgb) {
+    if (fuse_rgb && i == 0) {
       // last decoder conv with the RGB head (fusion.py:100-101,139) and the crop (eval/interpolator.py:175) in its
       // epilogue: the 64-channel activation is never written
       const size_t ci = add_conv(P, "fusion_conv2+rgb@L0", 9.0 * nf * nf + 64.0 * 3, M.fus_c2[i], {{f1, 0}}, 1, nullptr, 0,
@@ -1176,7 +1227,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
   }
   {
     const float *rw = M.rgb_w, *rb = M.rgb_b;
-    if (!(P.conv_impl == 0 && P.conv3x3_v2 && P.fuse_rgb_head && !keep_debug))
+    if (!fuse_rgb)
       P.add_op(2, "rgb_head", [=](cudaStream_t st) {
         return launch_rgb_head(net->hi, net->lo, net->C, pp->H, pp->W, rw, rb, pp->xout, (int64_t)pp->w * 3, pp->off_y,
                                pp->off_x, pp->h, pp->w, st);
@@ -1222,7 +1273,6 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
   FILM_CUDA(cudaMalloc(&P.d_probs, P.h_probs.size() * sizeof(ConvProblem)));
   P.allocs.push_back(P.d_probs);
   FILM_CUDA(cudaMemcpy(P.d_probs, P.h_probs.data(), P.h_probs.size() * sizeof(ConvProblem), cudaMemcpyHostToDevice));
-  (void)keep_debug;
   return pl;
 }
 
@@ -1238,10 +1288,10 @@ struct film_handle {
   cudaStream_t stream = nullptr;
   cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
   std::unique_ptr<Model> model;
-  std::map<std::string, std::unique_ptr<Plan>> plans;
+  std::map<std::vector<int>, std::unique_ptr<Plan>> plans;  // key: h, w, align, every plan-key option (get_plan)
   Plan* last_plan = nullptr;
   std::string err;
-  int conv_impl = 0, use_graph = 1, keep_debug = 0, time_ops = 0;
+  Options opt;
   bool dev_events_valid = false;  // ev[1]/ev[2] bracket the last device-pointer call
   cudaStream_t copy_stream = nullptr;   // H2D / D2H of tile t+1 / t-1 overlaps the network call of tile t
   float* stage_in[2] = {nullptr, nullptr};
@@ -1252,22 +1302,6 @@ struct film_handle {
   cudaStream_t lane_streams[Plan::kNumLanes] = {};  // lane 0 = the origin stream of the call
   std::vector<cudaEvent_t> token_events;
   cudaEvent_t fork_event = nullptr;
-  int use_lanes = 0;   // stream lanes measured no gain at 1080p (smem-saturating kernels cannot co-reside)
-  int conv3x3_v2 = 1;  // persistent tap-reuse kernel for 3x3 convs
-  int conv3x3_2cta = 0;  // CTA-pair clusters for the streamed-weight 3x3 convs of the large levels: off by default, 1080p
-                         // step 60.5 ms with them against 53.4 ms without (H100 SXM, 400 W; the paired layers run slower)
-  int conv3x3_halo = 3;  // wide halo boxes (one 10-px box per chunk serves nine taps): 0 off, 1 the CTA-pair layers, 2 every
-                         // 64-channel-chunk layer of the persistent kernel, 3 also its 32-channel-chunk layers
-  uint32_t onepass_mask = kDefaultOnepassMask;  // precision plan (see `enum Stage`)
-  int fe_conv0_tc = 0;  // cfeat_conv_0: 0 = register-tiled fp32 FMA kernel straight from the fp32 image (default: exact fp32,
-                        // no widened image tensor; K = 27 is not tensor-core work), 1 = tensor-core kernel over the
-                        // 32-channel-padded image
-  int fuse_rgb_head = 1;  // 1 = RGB head + crop in the epilogue of fusion_conv2@L0 (default), 0 = separate kernel
-  int plane_skip = 1, mma_straight = 1, arena_reuse = 1;   // optimisations, individually switchable (A/B, bisecting)
-  int fuse_flow_head = 1;
-  int conv3x3_pxn = 1;  // pixels on N for the Cout = 64 persistent 3x3 layers: 0 off, 1 where 32x8 tiles give two waves
-                        // over the SMs (default), 2 every eligible layer
-  int any_size = 0;     // 1: run padded sizes that are not multiples of 64 (levels with odd sizes), 0: refuse them
   uint8_t* u8_stage = nullptr;  // film_interpolate_u8: [x0][x1][out] on the device
   size_t u8_bytes = 0;
   int num_sms = 132;
@@ -1296,7 +1330,7 @@ static int fail(film_handle* h, const Error& e) noexcept {
 // cross-lane dependencies with events, join everything back into `origin`.  Works both eagerly and
 // under stream capture (the events become graph edges).
 static void enqueue_plan(film_handle* h, Plan* P, cudaStream_t origin) {
-  if (!h->use_lanes) {
+  if (!h->opt.use_lanes) {
     for (auto& op : P->ops) FILM_CUDA(op.fn(origin));
     return;
   }
@@ -1335,39 +1369,32 @@ static void drop_plans(film_handle* h) {
 }
 
 static Plan* get_plan(film_handle* h, int hh, int ww, int align) {
-  // Checked before the cache lookup: a plan built while "any_size" was 1 must not keep serving its size after the
+  // Checked before the cache lookup: a plan built while any_size was 1 must not keep serving its size after the
   // option is set back to 0.  The plan itself does not depend on the option.
-  if (!h->any_size) {
+  if (!h->opt.any_size) {
     int H, W, oy, ox;
     padded_size(hh, ww, align, H, W, oy, ox);
     if (H % 64 || W % 64)
       throw Error{FILM_ERR_UNSUPPORTED,
                   "padded frame size must be a multiple of 64 (2^(pyramid_levels-1)) in this engine; use align=64"};
   }
-  char key[96];
-  snprintf(key, sizeof(key), "%dx%d_a%d_i%d_v%d_l%d_p%d_h%d_m%x_d%d", hh, ww, align > 0 ? align : 0, h->conv_impl, h->conv3x3_v2,
-           h->use_lanes, h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->conv3x3_pxn * 512 + h->keep_debug * 256 + h->fuse_flow_head * 64 + h->arena_reuse * 32 + h->mma_straight * 16 + h->plane_skip * 8 +
-               h->fuse_rgb_head * 2 + h->fe_conv0_tc);
+  std::vector<int> key = {hh, ww, align > 0 ? align : 0};
+  for (const OptionRow& r : kOptions)
+    if (r.plan_key) key.push_back(h->opt.*r.field);
   auto it = h->plans.find(key);
   if (it != h->plans.end()) return it->second.get();
+  auto build = [&] { return build_plan(*h->model, hh, ww, align, h->opt, h->num_sms); };
   std::unique_ptr<Plan> p;
   try {
-    p = build_plan(*h->model, hh, ww, align, h->conv_impl, h->keep_debug != 0, h->conv3x3_v2, h->num_sms,
-                   h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->use_lanes != 0, h->fe_conv0_tc | (h->fuse_rgb_head ? 0 : 2) | (h->plane_skip ? 0 : 8) |
-                       (h->mma_straight ? 0 : 16) | (h->arena_reuse ? 0 : 32) | (h->fuse_flow_head ? 0 : 64) |
-                       (h->fuse_flow_head >= 2 ? 128 : 0) | (h->conv3x3_pxn << 8));
+    p = build();
   } catch (const Error& e0) {
-    if (e0.code != FILM_ERR_CUDA) throw;  // only an allocation failure is worth a retry
-    // Every cached shape keeps its activation arena (GBs at 1080p).  If a new shape does not fit next to
-    // them, drop the cache and retry once before giving up.
-    if (h->plans.empty()) throw;
+    // Only an allocation failure is worth a retry.  Every cached shape keeps its activation arena (GBs at 1080p).  If a
+    // new shape does not fit next to them, drop the cache and retry once before giving up.
+    if (e0.code != FILM_ERR_CUDA || h->plans.empty()) throw;
     drop_plans(h);
-    p = build_plan(*h->model, hh, ww, align, h->conv_impl, h->keep_debug != 0, h->conv3x3_v2, h->num_sms,
-                   h->conv3x3_2cta, h->conv3x3_halo, h->onepass_mask, h->use_lanes != 0, h->fe_conv0_tc | (h->fuse_rgb_head ? 0 : 2) | (h->plane_skip ? 0 : 8) |
-                       (h->mma_straight ? 0 : 16) | (h->arena_reuse ? 0 : 32) | (h->fuse_flow_head ? 0 : 64) |
-                       (h->fuse_flow_head >= 2 ? 128 : 0) | (h->conv3x3_pxn << 8));
+    p = build();
   }
-  if (h->use_graph) {
+  if (h->opt.use_graph) {
     cudaGraph_t g = nullptr;
     FILM_CUDA(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
     try {
@@ -1389,10 +1416,10 @@ static Plan* get_plan(film_handle* h, int hh, int ww, int align) {
 
 // runs the network of plan P on its xin -> xout (stream-ordered, not synchronised)
 static void run_plan(film_handle* h, Plan* P, cudaStream_t st) {
-  if (P->graph && !h->time_ops) {  // a captured graph can be replayed on any stream
+  if (P->graph && !h->opt.time_ops) {  // a captured graph can be replayed on any stream
     FILM_CUDA(cudaGraphLaunch(P->graph, st));
   } else {
-    if (h->time_ops && st == h->stream) {
+    if (h->opt.time_ops && st == h->stream) {
       // timed eager run: one event pair per op (bench.py's live per-kernel roofline numbers)
       const size_t n = P->ops.size();
       while (h->op_events.size() < n + 1) {
@@ -1447,15 +1474,9 @@ int film_create(film_handle** out, const char* weights_path, int device_ordinal)
     for (auto& e : h->ev) FILM_CUDA(cudaEventCreate(&e));
     FILM_CUDA(conv_tc_configure());
     FILM_CUDA(conv3x3_tc_configure());
-    if (const char* e2 = getenv("FILM_2CTA")) h->conv3x3_2cta = atoi(e2);
-    if (const char* e3 = getenv("FILM_HALO")) h->conv3x3_halo = atoi(e3);
-    if (const char* e5 = getenv("FILM_FE0_TC")) h->fe_conv0_tc = atoi(e5) ? 1 : 0;
-    if (const char* e6 = getenv("FILM_RGB_FUSE")) h->fuse_rgb_head = atoi(e6) ? 1 : 0;
-    if (const char* e8 = getenv("FILM_PLANE_SKIP")) h->plane_skip = atoi(e8) ? 1 : 0;
-    if (const char* e11 = getenv("FILM_FLOW_HEAD_FUSE")) h->fuse_flow_head = atoi(e11) < 0 ? 0 : (atoi(e11) > 2 ? 2 : atoi(e11));
-    if (const char* e9 = getenv("FILM_STRAIGHT")) h->mma_straight = atoi(e9) ? 1 : 0;
-    if (const char* e10 = getenv("FILM_ARENA_REUSE")) h->arena_reuse = atoi(e10) ? 1 : 0;
-    if (const char* e4 = getenv("FILM_ONEPASS")) h->onepass_mask = (uint32_t)strtoul(e4, nullptr, 0);
+    for (const OptionRow& r : kOptions)
+      if (const char* e = r.env ? getenv(r.env) : nullptr)  // a stage mask may be written in hex
+        h->opt.*r.field = r.normalise(r.field == &Options::onepass_mask ? (int)strtoul(e, nullptr, 0) : atoi(e));
     h->num_sms = prop.multiProcessorCount;
     WeightMap w = read_weight_file(weights_path);
     h->model.reset(new Model);
@@ -1507,31 +1528,13 @@ const char* film_last_error(film_handle* h) { return h ? h->err.c_str() : g_crea
 int film_set_option(film_handle* h, const char* name, int value) {
   if (!h || !name) return FILM_ERR_ARG;
   try {
-  std::string n(name);
-  if (n == "conv_impl") h->conv_impl = value;
-  else if (n == "use_graph") h->use_graph = value;
-  else if (n == "keep_debug") h->keep_debug = value;
-  else if (n == "time_ops") h->time_ops = value;
-  else if (n == "use_lanes") h->use_lanes = value;
-  else if (n == "conv3x3_v2") h->conv3x3_v2 = value;
-  else if (n == "conv3x3_2cta") h->conv3x3_2cta = value;
-  else if (n == "conv3x3_halo") h->conv3x3_halo = value;
-  else if (n == "onepass_mask") h->onepass_mask = (uint32_t)value & ((1u << ST_COUNT) - 1u);
-  else if (n == "onepass_default") h->onepass_mask = kDefaultOnepassMask;
-  else if (n == "fe_conv0_tc") h->fe_conv0_tc = value ? 1 : 0;
-  else if (n == "fuse_rgb_head") h->fuse_rgb_head = value ? 1 : 0;
-  else if (n == "plane_skip") h->plane_skip = value ? 1 : 0;
-  else if (n == "fuse_flow_head") h->fuse_flow_head = value < 0 ? 0 : (value > 2 ? 2 : value);
-  else if (n == "mma_straight") h->mma_straight = value ? 1 : 0;
-  else if (n == "conv3x3_pxn") h->conv3x3_pxn = value < 0 ? 0 : (value > 2 ? 2 : value);
-  else if (n == "arena_reuse") h->arena_reuse = value ? 1 : 0;
-  else if (n == "any_size") h->any_size = value ? 1 : 0;
-  else if (n == "clear_plans") drop_plans(h);
-  else {
-    h->err = "unknown option " + n;
-    return FILM_ERR_ARG;
-  }
-  return FILM_OK;
+    if (!strcmp(name, "onepass_default")) h->opt.onepass_mask = (int)kDefaultOnepassMask;
+    else if (!strcmp(name, "clear_plans")) drop_plans(h);
+    else {
+      const OptionRow& r = option_row(name);
+      h->opt.*r.field = r.normalise(value);
+    }
+    return FILM_OK;
   }
   FILM_CATCH_ALL(h)
 }
@@ -1551,15 +1554,11 @@ int film_stage_name(int stage, char* buf, int buf_size) {
 
 int film_get_option(film_handle* h, const char* name, int* value) {
   if (!h || !name || !value) return FILM_ERR_ARG;
-  if (!strcmp(name, "onepass_mask")) *value = (int)h->onepass_mask;
-  else if (!strcmp(name, "onepass_default")) *value = (int)kDefaultOnepassMask;
-  else if (!strcmp(name, "conv3x3_halo")) *value = h->conv3x3_halo;
-  else if (!strcmp(name, "conv3x3_2cta")) *value = h->conv3x3_2cta;
-  else if (!strcmp(name, "conv3x3_pxn")) *value = h->conv3x3_pxn;
-  else if (!strcmp(name, "keep_debug")) *value = h->keep_debug;
-  else if (!strcmp(name, "any_size")) *value = h->any_size;
-  else return FILM_ERR_ARG;
-  return FILM_OK;
+  try {
+    *value = !strcmp(name, "onepass_default") ? (int)kDefaultOnepassMask : h->opt.*option_row(name).field;
+    return FILM_OK;
+  }
+  FILM_CATCH_ALL(h)
 }
 
 int film_synchronize(film_handle* h) {
@@ -1670,7 +1669,7 @@ int film_interpolate(film_handle* h, const float* x0, const float* x1, const flo
     Plan* P = get_plan(h, H, W, align);
     const size_t frame = (size_t)H * W * 3 * sizeof(float);
     float ms_net = 0, ms_h2d = 0, ms_d2h = 0;
-    if (B > 1 && !h->time_ops) {
+    if (B > 1 && !h->opt.time_ops) {
       // batch of pairs: uploads / downloads of neighbouring pairs overlap the network calls
       run_pipelined(h, P, B, frame,
                     [&](int b, float* d0, float* d1, cudaStream_t cs) {
@@ -1752,7 +1751,7 @@ int film_interpolate_tiled(film_handle* h, const float* x0, const float* x1, con
     Plan* P = get_plan(h, ph, pw, align);
     const size_t row = (size_t)pw * 3 * sizeof(float), full_row = (size_t)W * 3 * sizeof(float);
     float ms_net = 0, ms_h2d = 0, ms_d2h = 0;
-    if (block_h * block_w > 1 && !h->time_ops) {
+    if (block_h * block_w > 1 && !h->opt.time_ops) {
       // tiles in row-major order (eval/interpolator.py:199-202), each padded on its own; the strided
       // upload of tile t+1 and download of tile t-1 overlap the network call of tile t
       const size_t tile_bytes = (size_t)ph * pw * 3 * sizeof(float);

@@ -180,8 +180,8 @@ FILM_API int film_profile(film_handle* h, film_profile_t* out);
  *                   three-pass split product.  The default is a measured per-stage plan;
  *                   0 = every conv three-pass (fp32-grade).  "onepass_default" (any value) restores it. */
 FILM_API int film_set_option(film_handle* h, const char* name, int value);
-/* Reads back an integer option ("onepass_mask", "onepass_default", "conv3x3_halo", "conv3x3_2cta", "conv3x3_pxn",
- * "keep_debug", "any_size"). */
+/* Reads back any value option of film_set_option, as stored (booleans as 0/1, clamped and masked values after the
+ * clamp or mask), or "onepass_default": the default precision plan.  An unknown name returns FILM_ERR_ARG. */
 FILM_API int film_get_option(film_handle* h, const char* name, int* value);
 
 /* Stages of the precision plan: film_stage_count() names ("fe_i0_k01", "flow_L3", "fus2_c1", ...), index =
