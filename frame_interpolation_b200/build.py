@@ -18,7 +18,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 SOURCES = ["film_engine.cu", "film_kernels.cu", "film_conv_tc.cu", "film_conv3x3_tc.cu"]
-HEADERS = ["film_common.cuh", "film_conv.h", "film_kernels.h", "film_tc_ptx.cuh", os.path.join("..", "..", "include", "film_b200.h")]
+HEADERS = ["film_common.cuh", "film_conv.h", "film_kernels.h", "film_pack.h", "film_tc_ptx.cuh", os.path.join("..", "..", "include", "film_b200.h")]
 LIB = os.path.join(HERE, "libfilm_b200.so")
 STAMP = os.path.join(HERE, "_build", "stamp")
 # ptxas remark (C75xx) for a kernel whose wgmma instructions it had to serialise; the build fails on it

@@ -72,7 +72,8 @@ __host__ __device__ inline int w_tap_bytes(int bn, int kc, int planes = 2) { ret
 
 // Variants are template parameters chosen on the host (launch_conv3x3_tc): kPartial = the activation stages
 // [v2_part_lo, v2_part_hi) of every tile read a source whose chunks hold data in their first 16-channel k-step only (the
-// 10-of-64 "side" source, the 3-of-32 image block); the all-zero k-steps are skipped; kHalo = wide halo boxes; kOne =
+// 10-of-64 "side" source, the 3-of-32 image block); the all-zero k-steps are skipped, and with kPxN the source's weights
+// come packed one K block per dx column (film_pack.h), so each block serves three taps; kHalo = wide halo boxes; kOne =
 // single-pass product A_hi x W_hi (hi planes only); kRes = resident weights issued as straight-line code (a whole
 // activation stage is one wgmma group); kPxN = pixels on N (BN = 64, KC = 64, 32x8 tiles, store / pool epilogue only).
 template <int BN, int KC, bool kPartial, bool kHalo, bool kOne, bool kRes, bool kPxN = false>
@@ -103,8 +104,16 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
   const int cout = prob->cout;
   const int n_nt = (cout + BN - 1) / BN;                       // N tiles (Cout = 512 -> 2)
   const int ntiles = prob->B * tiles_per_img * n_nt;            // work items (spatial, N), N fastest
-  int nkb = 0;                                                  // K blocks = (source, chunk, dx, dy)
-  for (int s = 0; s < nsrc; ++s) nkb += prob->src[s].nchunk * 9;
+  constexpr int kStageTaps = kHalo ? 9 : 3;                     // taps served by one activation stage
+  // Pixels on N: the partial source's packed weight blocks each hold k-step 0 of the three dy taps of one dx column.
+  // The 16x8 form keeps one block per tap: packing measured no faster there, and it made the BN = 128 and 256 partial
+  // instantiations spill about three times as much
+  constexpr bool kPacked = kPartial && kPxN;
+  const int part_lo = prob->v2_part_lo, part_hi = prob->v2_part_hi;   // kPartial: 1-k-step stages
+  int nab = 0;                                                  // activation stages: one halo box or three dx boxes per chunk
+  for (int s = 0; s < nsrc; ++s) nab += prob->src[s].nchunk * (kHalo ? 1 : 3);
+  // K blocks, in consumption order (source, chunk, dx, dy): one per tap, one per three taps in a packed partial stage
+  const int nkb = nab * kStageTaps - (kPacked ? (part_hi - part_lo) * (kStageTaps - kStageTaps / 3) : 0);
 
   const FastDiv div_nt(n_nt, ntiles), div_img(tiles_per_img, ntiles), div_tx(tiles_x, ntiles);   // tile decode
   // CTA pair (prob->pair, launched as (2,1,1) clusters): the two CTAs of a cluster walk the same work list, each on its
@@ -206,7 +215,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
         }
         __syncwarp();
       }
-      int kb = 0;
+      int kb = 0, ab = 0;
       for (int s = 0; s < nsrc; ++s) {
         const int nchunk = src_tab[2 * s], c_off = src_tab[2 * s + 1];
         const int bs = src_tab[2 * kMaxSrc + s] ? prob->B - 1 - b : b;
@@ -214,7 +223,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
         const CUtensorMap* tm_lo = &prob->tm_a_lo[s];
         for (int ch = 0; ch < nchunk; ++ch) {
           const int nst = halo ? 1 : 3;   // activation stages of this chunk: one wide halo box or three dx boxes
-          for (int dx = 0; dx < nst; ++dx) {
+          for (int dx = 0; dx < nst; ++dx, ++ab) {
             const int st = ra.stage;
             mbar_wait(tail + 8u * (kMaxRing + st), ra.phase ^ 1u);
             if (elect_one()) {
@@ -226,8 +235,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
             __syncwarp();
             ra.advance(NA);
             if (!resident) {
-              const int ntap = halo ? 9 : 3;   // weight taps consumed against this activation stage
-              for (int t = 0; t < ntap; ++t, ++kb) {
+              // weight blocks consumed against this activation stage: one per tap, one per dx column when packed
+              const bool packed = kPacked && ab >= part_lo && ab < part_hi;
+              const int nblk = packed ? kStageTaps / 3 : kStageTaps;
+              for (int t = 0; t < nblk; ++t, ++kb) {
                 const int ws = rw.stage;
                 mbar_wait(tail + 8u * (3 * kMaxRing + ws), rw.phase ^ 1u);
                 if (elect_one()) {
@@ -303,10 +314,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
   };
   {
     constexpr int kWTapC = kWPlane * (kOne ? 1 : 2);
-    constexpr int kStageTaps = kHalo ? 9 : 3;   // taps served by one activation stage
     constexpr uint32_t kPx = KC * 2;            // bytes of one pixel row of a box
-    const int nab = nkb / kStageTaps;           // activation stages per tile
-    [[maybe_unused]] const int part_lo = prob->v2_part_lo, part_hi = prob->v2_part_hi;   // kPartial: 1-k-step stages
     // first pixel row of this warpgroup's pixels inside the box, and the stride between its 8-row groups
     const uint32_t a_row0 = kHalo ? (uint32_t)(wg * (kWgPx / 8) * kHaloW) * kPx : (uint32_t)(wg * kWgPx) * kPx;
     const uint32_t sbo = kHalo ? kHaloW * kPx : 8 * kPx;
@@ -326,9 +334,11 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
         rel_w = next_w;
       };
       // One activation stage whose products each issue kSteps k-steps (a compile-time count: ptxas serialises every
-      // wgmma of a kernel in which a runtime condition picks between wgmma sequences, C7520)
-      auto stage = [&](auto ksteps_c) {
-        constexpr int kSteps = decltype(ksteps_c)::value;
+      // wgmma of a kernel in which a runtime condition picks between wgmma sequences, C7520).  kTpb taps share one
+      // weight block, their k-steps back to back in it: 3 in a packed partial stage (k-step 0 of each dy tap), else 1
+      auto stage = [&](auto ksteps_c, auto tpb_c) {
+        constexpr int kSteps = decltype(ksteps_c)::value, kTpb = decltype(tpb_c)::value;
+        constexpr int kBlocks = kStageTaps / kTpb;   // weight blocks read against this stage
         const int st = ra.stage;
         mbar_wait(tail + 8u * st, ra.phase);
         const uint32_t sa = a_base + st * kAStage + a_row0;
@@ -346,7 +356,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
           for (int t = 0; t < kStageTaps; ++t) {
             const uint64_t a_hi = a0 + (kHalo ? (uint64_t)((((t % 3) * kHaloW + t / 3) * kPx) >> 4) : (uint64_t)t * row_delta);
             const uint64_t a_lo = a_hi + lo_delta;
-            const uint64_t w_hi = w0 + (uint64_t)((t * kWTapC) >> 4), w_lo = w_hi + (uint64_t)(kWPlane >> 4);
+            const uint64_t w_hi = w0 + (uint64_t)(((t / kTpb) * kWTapC + (t % kTpb) * kSteps * 32) >> 4);
+            const uint64_t w_lo = w_hi + (uint64_t)(kWPlane >> 4);
 #pragma unroll
             for (int k = 0; k < kSteps; ++k) {
               const uint64_t adv = (uint64_t)(k * 32 >> 4);
@@ -371,9 +382,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
             }
           }
           retire(st, -1);
-          kb += kStageTaps;
+          kb += kBlocks;
         } else {
-          for (int t = 0; t < kStageTaps; ++t, ++kb) {
+          for (int blk = 0; blk < kBlocks; ++blk, ++kb) {
             uint32_t sw;
             int ws = -1;
             if (resident) {
@@ -383,34 +394,40 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
               mbar_wait(tail + 8u * (2 * kMaxRing + ws), rw.phase);
               sw = w_base + ws * kWTap;
             }
-            const uint32_t off = kHalo ? (uint32_t)((t % 3) * kHaloW + t / 3) * kPx : (uint32_t)(t * kRowStep);
-            const uint64_t a_hi = make_desc_sbo<KC>(sa + off, sbo);
-            const uint64_t a_lo = make_desc_sbo<KC>(sa + lo_off + off, sbo);
-            const uint64_t w_hi = make_desc_kc<KC>(sw), w_lo = make_desc_kc<KC>(sw + kWPlane);
             const uint32_t first = (kb == 0) ? 0u : 1u;
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < kSteps; ++k) {
-              const uint64_t adv = (uint64_t)(k * 32 >> 4);
-              if constexpr (kPxN) {
-                wgmma<128>(acc, w_hi + adv, a_hi + adv, k == 0 ? first : 1u);
-                if constexpr (!kOne) {
-                  wgmma<128>(acc, w_lo + adv, a_hi + adv, 1u);
-                  wgmma<128>(acc, w_hi + adv, a_lo + adv, 1u);
+            for (int u = 0; u < kTpb; ++u) {
+              const int t = blk * kTpb + u;
+              const uint32_t off = kHalo ? (uint32_t)((t % 3) * kHaloW + t / 3) * kPx : (uint32_t)(t * kRowStep);
+              const uint64_t a_hi = make_desc_sbo<KC>(sa + off, sbo);
+              const uint64_t a_lo = make_desc_sbo<KC>(sa + lo_off + off, sbo);
+              const uint64_t wk = (uint64_t)((u * kSteps * 32) >> 4);   // the tap's first k-step inside the block
+              const uint64_t w_hi = make_desc_kc<KC>(sw) + wk, w_lo = make_desc_kc<KC>(sw + kWPlane) + wk;
+#pragma unroll
+              for (int k = 0; k < kSteps; ++k) {
+                const uint64_t adv = (uint64_t)(k * 32 >> 4);
+                const uint32_t accf = (u == 0 && k == 0) ? first : 1u;
+                if constexpr (kPxN) {
+                  wgmma<128>(acc, w_hi + adv, a_hi + adv, accf);
+                  if constexpr (!kOne) {
+                    wgmma<128>(acc, w_lo + adv, a_hi + adv, 1u);
+                    wgmma<128>(acc, w_hi + adv, a_lo + adv, 1u);
+                  }
+                } else if constexpr (kOne) {
+                  wgmma<BN>(acc, a_hi + adv, w_hi + adv, accf);
+                } else if constexpr (kFused) {
+                  wgmma<BN>(acc, a_hi + adv, w_hi + adv, accf);
+                  wgmma<BN>(acc + BN / 2, a_hi + adv, w_lo + adv, accf);
+                  wgmma<BN>(acc, a_lo + adv, w_hi + adv, 1u);
+                } else {
+                  wgmma<BN>(acc, a_lo + adv, w_hi + adv, accf);
+                  wgmma<BN>(acc, a_hi + adv, w_lo + adv, 1u);
+                  wgmma<BN>(acc, a_hi + adv, w_hi + adv, 1u);
                 }
-              } else if constexpr (kOne) {
-                wgmma<BN>(acc, a_hi + adv, w_hi + adv, k == 0 ? first : 1u);
-              } else if constexpr (kFused) {
-                wgmma<BN>(acc, a_hi + adv, w_hi + adv, k == 0 ? first : 1u);
-                wgmma<BN>(acc + BN / 2, a_hi + adv, w_lo + adv, k == 0 ? first : 1u);
-                wgmma<BN>(acc, a_lo + adv, w_hi + adv, 1u);
-              } else {
-                wgmma<BN>(acc, a_lo + adv, w_hi + adv, k == 0 ? first : 1u);
-                wgmma<BN>(acc, a_hi + adv, w_lo + adv, 1u);
-                wgmma<BN>(acc, a_hi + adv, w_hi + adv, 1u);
               }
             }
-            retire(t == kStageTaps - 1 ? st : -1, ws);
+            retire(blk == kBlocks - 1 ? st : -1, ws);
             if (!resident) rw.advance(NW);
           }
         }
@@ -418,12 +435,13 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
       };
       // the partial source's stages run in a loop of their own: no condition between alternative wgmma sequences
       using Full = std::integral_constant<int, KC / 16>;
+      using One = std::integral_constant<int, 1>;
       if constexpr (kPartial) {
-        for (int ab = 0; ab < part_lo; ++ab) stage(Full{});
-        for (int ab = part_lo; ab < part_hi; ++ab) stage(std::integral_constant<int, 1>{});
-        for (int ab = part_hi; ab < nab; ++ab) stage(Full{});
+        for (int ab = 0; ab < part_lo; ++ab) stage(Full{}, One{});
+        for (int ab = part_lo; ab < part_hi; ++ab) stage(One{}, std::integral_constant<int, kPacked ? 3 : 1>{});
+        for (int ab = part_hi; ab < nab; ++ab) stage(Full{}, One{});
       } else {
-        for (int ab = 0; ab < nab; ++ab) stage(Full{});
+        for (int ab = 0; ab < nab; ++ab) stage(Full{}, One{});
       }
       wgmma_wait<0>();
       if (is_leader) {

@@ -19,6 +19,7 @@
 #include "../../include/film_b200.h"
 #include "film_conv.h"
 #include "film_kernels.h"
+#include "film_pack.h"
 
 namespace film {
 int conv_tc_block_n(int cout);
@@ -88,7 +89,8 @@ struct Options {
   int conv3x3_halo = 3;  // wide halo boxes (one 10-px box per chunk serves nine taps): 0 off, 1 the CTA-pair layers, 2 every
                          // 64-channel-chunk layer of the persistent kernel, 3 also its 32-channel-chunk layers
   int conv3x3_pxn = 1;   // pixels on N for the Cout = 64 persistent 3x3 layers: 0 off, 1 where 32x8 tiles give two waves
-                         // over the SMs (default), 2 every eligible layer
+                         // over the SMs, k-step-skipping layers where they take half the waves of 16x8 tiles (default),
+                         // 2 every eligible layer
   int onepass_mask = (int)kDefaultOnepassMask;  // precision plan: stages on the single-pass product (see `enum Stage`)
   int fe_conv0_tc = 0;   // cfeat_conv_0: 0 = fp32 FMA kernel straight from the fp32 image (exact fp32, no widened image
                          // tensor; K = 27 is not tensor-core work), 1 = tensor-core kernel over the 32-channel-padded image
@@ -241,6 +243,11 @@ struct PackedConv {
   int kchunk = kChunk;          // channels per K block (64, or 32 for the 32-channel layers)
   std::vector<int> src_chunks;  // K-block chunks per source
   std::vector<int> src_ksteps;  // 16-channel k-steps per chunk that hold at least one real channel
+  // weights of the pixels-on-N 3x3 kernel: a one-k-step source with 64-channel chunks is packed one K block per dx
+  // column (film_pack.h); the same arrays as w_hi / w_lo when no source is packed
+  sp_t* pxn_hi = nullptr;
+  sp_t* pxn_lo = nullptr;
+  int pxn_ktot = 0;
   int ntaps = 0;
   int tap_dy[kMaxTaps], tap_dx[kMaxTaps];
 };
@@ -302,14 +309,26 @@ static PackedConv pack_conv(const HostTensor& kernel, const HostTensor& bias,
       }
     }
   }
-  FILM_CUDA(cudaMalloc(&pc.w_hi, hi.size() * 2));
-  allocs.push_back(pc.w_hi);
-  FILM_CUDA(cudaMalloc(&pc.w_lo, lo.size() * 2));
-  allocs.push_back(pc.w_lo);
+  auto upload = [&](const std::vector<uint16_t>& v) {
+    sp_t* d;
+    FILM_CUDA(cudaMalloc(&d, v.size() * 2));
+    allocs.push_back(d);
+    FILM_CUDA(cudaMemcpy(d, v.data(), v.size() * 2, cudaMemcpyHostToDevice));
+    return d;
+  };
+  pc.w_hi = upload(hi);
+  pc.w_lo = upload(lo);
+  pc.pxn_hi = pc.w_hi;
+  pc.pxn_lo = pc.w_lo;
+  pc.pxn_ktot = ktot;
+  std::vector<int> packed;
+  for (int ks : pc.src_ksteps) packed.push_back(taps.size() == 9 && chunk == kChunk && ks == 1);
+  if (std::count(packed.begin(), packed.end(), 1)) {
+    pc.pxn_hi = upload(pack_dx_blocks(hi, cout, ktot, chunk, pc.src_chunks, packed, pc.pxn_ktot));
+    pc.pxn_lo = upload(pack_dx_blocks(lo, cout, ktot, chunk, pc.src_chunks, packed, pc.pxn_ktot));
+  }
   FILM_CUDA(cudaMalloc(&pc.bias, cout * 4));
   allocs.push_back(pc.bias);
-  FILM_CUDA(cudaMemcpy(pc.w_hi, hi.data(), hi.size() * 2, cudaMemcpyHostToDevice));
-  FILM_CUDA(cudaMemcpy(pc.w_lo, lo.data(), lo.size() * 2, cudaMemcpyHostToDevice));
   FILM_CUDA(cudaMemcpy(pc.bias, bias.data.data(), cout * 4, cudaMemcpyHostToDevice));
   return pc;
 }
@@ -669,17 +688,23 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
                   (kc == kChunk || pc.cout <= 64);
   cp.epi_mode = epi_mode;
   // pixels on the wgmma N dimension (film_conv3x3_tc.cu): the Cout = 64 layers with 64-channel chunks and a plain or
-  // pooled store run on 32x8 tiles.  By default only where those still give two waves over the SMs, and not with a
-  // source that skips k-steps: fusion_conv1@L0 measured slower on the new form (4.26 -> 4.52 ms, H100 SXM, 400 W);
-  // its side-source stages issue one k-step per 16 KiB weight tap, and with 256-pixel tiles its streamed weight ring
-  // has only two slots
+  // pooled store run on 32x8 tiles.  By default only where those still give two waves over the SMs.  A layer with a
+  // source that skips k-steps (fusion_conv1) moves only where the 32x8 tiles take at most half the waves of 16x8 tiles.
+  // fusion_conv1@L0 at 1088x1920 (62 waves against 124): 2.39 against 3.47 ms (H100 SXM, 700 W).  At 256x320 (3
+  // against 5) it stays on 16x8 tiles; pixels on N measured 0.135 against 0.148 ms there, a gain this rule gives up
+  const auto waves = [&](long tiles) { return (tiles + P.num_sms - 1) / P.num_sms; };
   const long pxn_tiles = (long)cp.B * ((cp.H + 31) / 32) * ((cp.W + 7) / 8);
+  const long tiles16 = (long)cp.B * ((cp.H + 15) / 16) * ((cp.W + 7) / 8);
   bool skips_ksteps = false;
   for (size_t s = 0; s < pc.src_chunks.size(); ++s)
     if (pc.src_chunks[s] > 0 && pc.src_ksteps[s] != kc / 16) skips_ksteps = true;
+  const bool pxn_pays = skips_ksteps ? 2 * waves(pxn_tiles) <= waves(tiles16) : pxn_tiles >= 2L * P.num_sms;
   cp.pxn = (v2 && o.conv3x3_pxn && pc.cout == 64 && kc == kChunk && epi_mode == 0 && out && out_c_off % 8 == 0 &&
-            out->C % 8 == 0 && (!pool_out || pool_out->C % 8 == 0) &&
-            (o.conv3x3_pxn >= 2 || (pxn_tiles >= 2L * P.num_sms && !skips_ksteps))) ? 1 : 0;
+            out->C % 8 == 0 && (!pool_out || pool_out->C % 8 == 0) && (o.conv3x3_pxn >= 2 || pxn_pays)) ? 1 : 0;
+  // the pixels-on-N kernel reads a one-k-step source's weights packed per dx column, every other kernel per tap
+  const int ktot = cp.pxn ? pc.pxn_ktot : pc.ktot;
+  const sp_t* w_hi = cp.pxn ? pc.pxn_hi : pc.w_hi;
+  const sp_t* w_lo = cp.pxn ? pc.pxn_lo : pc.w_lo;
   int box_h, box_w;
   if (v2) {
     if (cp.pxn) {
@@ -689,7 +714,7 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
       cp.tile_h = 16;  // the fused pool of a 16x8 tile finds each 2x2 partner in lane ^ 4 and the thread's second fragment row
       cp.tile_w = 8;
     } else {
-      conv3x3_tc_pick_tile(cp.H, cp.W, cp.B, pc.cout, kc, cp.passes, pc.ktot, epi_mode, P.num_sms, cp.tile_h, cp.tile_w);
+      conv3x3_tc_pick_tile(cp.H, cp.W, cp.B, pc.cout, kc, cp.passes, ktot, epi_mode, P.num_sms, cp.tile_h, cp.tile_w);
     }
     box_h = cp.tile_h + 2;
     box_w = cp.tile_w;
@@ -718,9 +743,9 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
     cp.tap_dy[t] = pc.tap_dy[t];
     cp.tap_dx[t] = pc.tap_dx[t];
   }
-  cp.ktot = pc.ktot;
-  cp.w_hi = pc.w_hi;
-  cp.w_lo = pc.w_lo;
+  cp.ktot = ktot;
+  cp.w_hi = w_hi;
+  cp.w_lo = w_lo;
   cp.bias = pc.bias;
   cp.cout = pc.cout;
   cp.act = act;
@@ -732,10 +757,10 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
     while (bn > 64 && 2 * items(bn) <= P.num_sms) bn /= 2;  // only while under half of the SMs have work
   }
   cp.bn = bn;
-  make_w_map(&cp.tm_w_hi, pc.w_hi, pc.cout, pc.ktot, bn, kc);
-  make_w_map(&cp.tm_w_lo, pc.w_lo, pc.cout, pc.ktot, bn, kc);
-  make_w_map(&cp.tm_w_hi_half, pc.w_hi, pc.cout, pc.ktot, bn / 2, kc);
-  make_w_map(&cp.tm_w_lo_half, pc.w_lo, pc.cout, pc.ktot, bn / 2, kc);
+  make_w_map(&cp.tm_w_hi, w_hi, pc.cout, ktot, bn, kc);
+  make_w_map(&cp.tm_w_lo, w_lo, pc.cout, ktot, bn, kc);
+  make_w_map(&cp.tm_w_hi_half, w_hi, pc.cout, ktot, bn / 2, kc);
+  make_w_map(&cp.tm_w_lo_half, w_lo, pc.cout, ktot, bn / 2, kc);
   if (out) {
     cp.out_hi = out->hi;
     cp.out_lo = out->lo;
@@ -763,6 +788,10 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   // wide halo level: 1 = CTA-pair layers, 2 = + every persistent layer (64-channel chunks), 3 = + 32-channel chunks
   int halo_ok = (v2 && cp.tile_h == (cp.pxn ? 32 : 16) && cp.tile_w == 8) ? o.conv3x3_halo : 0;
   if (kc != kChunk && halo_ok < 3) halo_ok = 0;
+  // pixels on N with a source that skips k-steps: three dx boxes.  Two wide 32x8 halo stages leave the streamed weight
+  // ring two slots, too few to cover the light one-k-step stages; the smaller dx boxes leave it four.  fusion_conv1@L0
+  // at 1088x1920: 3.04 ms against 4.20 with the wide halo (H100 SXM, 400 W)
+  if (cp.pxn && skips_ksteps) halo_ok = 0;
   cp.halo = halo_ok >= 2;
   if (v2 && !conv3x3_tc_plan(cp, P.num_sms))
     throw Error{FILM_ERR_UNSUPPORTED, "persistent 3x3 conv: shared-memory rings do not fit (" + tag + ")"};
@@ -812,7 +841,7 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
     if (pool_out) alg_bytes += px / 4.0 * pc.cout * 4.0;
     if (epi_mode == 2) alg_bytes += px * 12.0;
     if (!out && epi_mode != 2) alg_bytes += px * 24.0;   // flow heads: v_up read, residual and flow written
-    alg_bytes += (double)pc.cout * pc.ktot * 2.0 * planes_in;
+    alg_bytes += (double)pc.cout * ktot * 2.0 * planes_in;
   }
   P.last_conv_bytes = alg_bytes;
   if (no_op) return idx;  // the caller launches this problem as part of a group

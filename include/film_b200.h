@@ -152,7 +152,8 @@ FILM_API int film_profile(film_handle* h, film_profile_t* out);
  *                   2 = 64-channel chunks only, 1 = CTA-pair layers only, 0 = three dx-shifted 8-px boxes
  *   "conv3x3_pxn" : persistent 3x3 layers with Cout = 64, 64-channel chunks and a plain or pooled store put the pixels
  *                   on the wgmma N dimension (m64n128k16, weight tap as the M operand, 32x8 tiles): 1 = where 32x8 tiles
- *                   still give two waves over the SMs and no source skips k-steps (default), 2 = every such layer, 0 = off
+ *                   still give two waves over the SMs, and for a layer with a source that skips k-steps (fusion conv_1)
+ *                   where they take at most half the waves of 16x8 tiles (default), 2 = every such layer, 0 = off
  *   "fe_conv0_tc" : cfeat_conv_0 (3 -> 64, K = 27): 0 = register-tiled fp32 FMA kernel reading the fp32 image directly
  *                   (default: exact fp32 arithmetic, no widened image tensor), 1 = tensor-core kernel over a 32-channel-
  *                   padded split image
