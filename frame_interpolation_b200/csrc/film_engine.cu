@@ -100,11 +100,14 @@ struct Options {
   int mma_straight = 1;  // straight-line MMA issue for resident weights
   int arena_reuse = 1;   // activation buffers are recycled inside a plan by liveness
   int any_size = 0;      // 1: run padded sizes that are not multiples of 64 (levels with odd sizes), 0: refuse them
+  int tile_overlap = 0;  // film_interpolate_tiled: pixels each tile's window reaches past interior tile boundaries, with a
+                         // feathered stitch over them; 0 = the reference's non-overlapping tiles, pasted
 };
 
 static int as_given(int v) { return v; }
 static int as_bool(int v) { return v ? 1 : 0; }
 static int clamp_0_2(int v) { return v < 0 ? 0 : (v > 2 ? 2 : v); }
+static int non_negative(int v) { return v < 0 ? 0 : v; }
 static int stage_bits(int v) { return (int)((uint32_t)v & ((1u << ST_COUNT) - 1u)); }
 struct OptionRow {
   const char* name;
@@ -132,6 +135,8 @@ static const OptionRow kOptions[] = {
     {"arena_reuse", &Options::arena_reuse, as_bool, "FILM_ARENA_REUSE", true},
     // only decides whether a size is accepted (get_plan, before the cache lookup): a 64-aligned size runs the same plan
     {"any_size", &Options::any_size, as_bool, nullptr, false},
+    // not a plan key: the window shape it gives film_interpolate_tiled already selects the plan
+    {"tile_overlap", &Options::tile_overlap, non_negative, nullptr, false},
 };
 static const OptionRow& option_row(const char* name) {
   for (const OptionRow& r : kOptions)
@@ -1333,6 +1338,8 @@ struct film_handle {
   cudaEvent_t fork_event = nullptr;
   uint8_t* u8_stage = nullptr;  // film_interpolate_u8: [x0][x1][out] on the device
   size_t u8_bytes = 0;
+  float* overlap_stage = nullptr;  // film_interpolate_tiled with tile_overlap > 0: [x0][x1][out][window results]
+  size_t overlap_bytes = 0;
   int num_sms = 132;
   std::vector<cudaEvent_t> op_events;
   film_profile_t prof;
@@ -1544,6 +1551,7 @@ void film_destroy(film_handle* h) {
       if (e) cudaEventDestroy(e);
   }
   if (h->u8_stage) cudaFree(h->u8_stage);
+  if (h->overlap_stage) cudaFree(h->overlap_stage);
   if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
   if (h->fork_event) cudaEventDestroy(h->fork_event);
   for (int i = 1; i < Plan::kNumLanes; ++i)
@@ -1735,6 +1743,19 @@ int film_interpolate(film_handle* h, const float* x0, const float* x1, const flo
   FILM_CATCH_ALL(h)
 }
 
+// One network call on row-pitched device views, staged through the plan's fixed input / output buffers so that the
+// captured graph stays pointer-stable.  ev[1] / ev[2] bracket the network.
+static void run_on_views(film_handle* h, Plan* P, const float* d_x0, const float* d_x1, int H, int W, int64_t in_pitch,
+                         float* d_out, int64_t out_pitch, cudaStream_t st) {
+  const size_t row = (size_t)W * 3 * sizeof(float);
+  FILM_CUDA(cudaMemcpy2DAsync(P->xin, row, d_x0, in_pitch * 4, row, H, cudaMemcpyDeviceToDevice, st));
+  FILM_CUDA(cudaMemcpy2DAsync(P->xin + (int64_t)H * W * 3, row, d_x1, in_pitch * 4, row, H, cudaMemcpyDeviceToDevice, st));
+  FILM_CUDA(cudaEventRecord(h->ev[1], st));
+  run_plan(h, P, st);
+  FILM_CUDA(cudaEventRecord(h->ev[2], st));
+  FILM_CUDA(cudaMemcpy2DAsync(d_out, out_pitch * 4, P->xout, row, row, H, cudaMemcpyDeviceToDevice, st));
+}
+
 int film_interpolate_device(film_handle* h, const float* d_x0, const float* d_x1, int B, int H, int W,
                             int64_t in_pitch, int align, float* d_out, int64_t out_pitch, void* cuda_stream) {
   if (!h) return FILM_ERR_ARG;
@@ -1745,24 +1766,96 @@ int film_interpolate_device(film_handle* h, const float* d_x0, const float* d_x1
     (void)cudaGetLastError();
     Plan* P = get_plan(h, H, W, align);
     cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : h->stream;
-    const size_t row = (size_t)W * 3 * sizeof(float);
-    for (int b = 0; b < B; ++b) {
-      // stage into the plan's fixed input buffers so the captured graph stays pointer-stable
-      FILM_CUDA(cudaMemcpy2DAsync(P->xin, row, d_x0 + (int64_t)b * H * in_pitch, in_pitch * 4, row, H,
-                                  cudaMemcpyDeviceToDevice, st));
-      FILM_CUDA(cudaMemcpy2DAsync(P->xin + (int64_t)H * W * 3, row, d_x1 + (int64_t)b * H * in_pitch, in_pitch * 4, row, H,
-                                  cudaMemcpyDeviceToDevice, st));
-      FILM_CUDA(cudaEventRecord(h->ev[1], st));
-      run_plan(h, P, st);
-      FILM_CUDA(cudaEventRecord(h->ev[2], st));
-      FILM_CUDA(cudaMemcpy2DAsync(d_out + (int64_t)b * H * out_pitch, out_pitch * 4, P->xout, row, row, H,
-                                  cudaMemcpyDeviceToDevice, st));
-    }
+    for (int b = 0; b < B; ++b)
+      run_on_views(h, P, d_x0 + (int64_t)b * H * in_pitch, d_x1 + (int64_t)b * H * in_pitch, H, W, in_pitch,
+                   d_out + (int64_t)b * H * out_pitch, out_pitch, st);
     fill_profile(h, P, -1.f, 0.f, 0.f);
     h->dev_events_valid = true;
     return FILM_OK;
   }
   FILM_CATCH_ALL(h)
+}
+
+// Overlapped tiling (option tile_overlap), the geometry of spec.tile_windows restated: every window of an axis cut into
+// b > 1 blocks has the length p + 2v and border windows are shifted inward, so one frame needs one plan.
+static StitchAxis stitch_axis(const char* name, int L, int b, int overlap) {
+  StitchAxis a;
+  a.b = b, a.L = L, a.p = L / b;
+  a.v = b > 1 ? overlap : 0;
+  a.q = a.p + 2 * a.v;
+  if (2 * a.v > a.p)  // the ramps of consecutive boundaries would meet: a pixel could see three windows
+    throw Error{FILM_ERR_ARG, "tile_overlap=" + std::to_string(overlap) + " is more than half the tile " + name + "=" +
+                                  std::to_string(a.p) + "."};
+  return a;
+}
+
+static StitchGeom stitch_geometry(int H, int W, int block_h, int block_w, int overlap, const int* slot_of_tile) {
+  if (H < 1 || W < 1) throw Error{FILM_ERR_ARG, "height and width must be positive"};
+  if (block_h < 1 || block_w < 1) throw Error{FILM_ERR_ARG, "block shape must be positive"};
+  if (H % block_h) throw Error{FILM_ERR_ARG, "block_height=" + std::to_string(block_h) + " should evenly divide height=" + std::to_string(H) + "."};
+  if (W % block_w) throw Error{FILM_ERR_ARG, "block_width=" + std::to_string(block_w) + " should evenly divide width=" + std::to_string(W) + "."};
+  if (overlap < 0) throw Error{FILM_ERR_ARG, "tile overlap must not be negative"};
+  if ((int64_t)block_h * block_w > kMaxStitchTiles)
+    throw Error{FILM_ERR_ARG, "the feathered stitch takes at most " + std::to_string(kMaxStitchTiles) + " tiles"};
+  if (H > 65535) throw Error{FILM_ERR_ARG, "the feathered stitch takes frames of at most 65535 rows"};
+  StitchGeom g;
+  g.ay = stitch_axis("height", H, block_h, overlap);
+  g.ax = stitch_axis("width", W, block_w, overlap);
+  for (int t = 0; t < kMaxStitchTiles; ++t) {
+    g.slot[t] = t < block_h * block_w && slot_of_tile ? slot_of_tile[t] : t;
+    if (g.slot[t] < 0) throw Error{FILM_ERR_ARG, "negative slot in slot_of_tile"};
+  }
+  return g;
+}
+
+int film_stitch_tiles_device(film_handle* h, const float* d_tiles, int64_t tile_stride, const int* slot_of_tile, int H,
+                             int W, int block_h, int block_w, int overlap, float* d_out, int64_t out_pitch,
+                             void* cuda_stream) {
+  if (!h) return FILM_ERR_ARG;
+  try {
+    if (!d_tiles || !d_out) throw Error{FILM_ERR_ARG, "null tile or frame pointer"};
+    const StitchGeom g = stitch_geometry(H, W, block_h, block_w, overlap, slot_of_tile);
+    if (tile_stride < (int64_t)g.ay.q * g.ax.q * 3) throw Error{FILM_ERR_ARG, "tile_stride smaller than a window"};
+    if (out_pitch < (int64_t)W * 3) throw Error{FILM_ERR_ARG, "pitch smaller than a row"};
+    FILM_CUDA(cudaSetDevice(h->device));
+    (void)cudaGetLastError();
+    FILM_CUDA(launch_stitch_feather(d_tiles, tile_stride, g, d_out, out_pitch,
+                                    cuda_stream ? (cudaStream_t)cuda_stream : h->stream));
+    return FILM_OK;
+  }
+  FILM_CATCH_ALL(h)
+}
+
+// film_interpolate_tiled with tile_overlap > 0: both frames are uploaded once, every window runs as a pitched view of
+// the resident frames into a [tiles][q_h][q_w][3] buffer, one kernel stitches that buffer into a device frame, one
+// download.  The scratch memory belongs to the handle.
+static void interpolate_tiled_overlapped(film_handle* h, const float* x0, const float* x1, int H, int W, int align,
+                                         int block_h, int block_w, float* out) {
+  const StitchGeom g = stitch_geometry(H, W, block_h, block_w, h->opt.tile_overlap, nullptr);
+  const int qh = g.ay.q, qw = g.ax.q, nt = block_h * block_w;
+  (void)cudaGetLastError();
+  Plan* P = get_plan(h, qh, qw, align);
+  const size_t frame = (size_t)H * W * 3, window = (size_t)qh * qw * 3;  // floats
+  const size_t need = (3 * frame + nt * window) * sizeof(float);
+  if (h->overlap_bytes < need) {
+    if (h->overlap_stage) cudaFree(h->overlap_stage);
+    h->overlap_stage = nullptr;
+    h->overlap_bytes = 0;
+    FILM_CUDA(cudaMalloc(&h->overlap_stage, need));
+    h->overlap_bytes = need;
+  }
+  float *d0 = h->overlap_stage, *d1 = d0 + frame, *d_out = d1 + frame, *d_tiles = d_out + frame;
+  cudaStream_t st = h->stream;
+  FILM_CUDA(cudaMemcpyAsync(d0, x0, frame * sizeof(float), cudaMemcpyHostToDevice, st));
+  FILM_CUDA(cudaMemcpyAsync(d1, x1, frame * sizeof(float), cudaMemcpyHostToDevice, st));
+  for (int t = 0; t < nt; ++t) {  // row-major tile order, like the non-overlapping path
+    const size_t off = ((size_t)stitch_origin(g.ay, t / block_w) * W + stitch_origin(g.ax, t % block_w)) * 3;
+    run_on_views(h, P, d0 + off, d1 + off, qh, qw, (int64_t)W * 3, d_tiles + t * window, (int64_t)qw * 3, st);
+  }
+  FILM_CUDA(launch_stitch_feather(d_tiles, (int64_t)window, g, d_out, (int64_t)W * 3, st));
+  FILM_CUDA(cudaMemcpyAsync(out, d_out, frame * sizeof(float), cudaMemcpyDeviceToHost, st));
+  FILM_CUDA(cudaStreamSynchronize(st));
+  fill_profile(h, P, 0.f, 0.f, 0.f);
 }
 
 int film_interpolate_tiled(film_handle* h, const float* x0, const float* x1, const float* dt, int H, int W, int align,
@@ -1776,6 +1869,10 @@ int film_interpolate_tiled(film_handle* h, const float* x0, const float* x1, con
     if (H % block_h) throw Error{FILM_ERR_ARG, "block_height=" + std::to_string(block_h) + " should evenly divide height=" + std::to_string(H) + "."};
     if (W % block_w) throw Error{FILM_ERR_ARG, "block_width=" + std::to_string(block_w) + " should evenly divide width=" + std::to_string(W) + "."};
     FILM_CUDA(cudaSetDevice(h->device));
+    if (h->opt.tile_overlap > 0 && block_h * block_w > 1) {
+      interpolate_tiled_overlapped(h, x0, x1, H, W, align, block_h, block_w, out);
+      return FILM_OK;
+    }
     const int ph = H / block_h, pw = W / block_w;
     Plan* P = get_plan(h, ph, pw, align);
     const size_t row = (size_t)pw * 3 * sizeof(float), full_row = (size_t)W * 3 * sizeof(float);

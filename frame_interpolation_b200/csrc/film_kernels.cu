@@ -115,6 +115,106 @@ cudaError_t launch_f32_to_u8(const float* src, uint8_t* dst, int64_t n, cudaStre
 }
 
 // ------------------------------------------------------------------------------------------
+// Feathered stitch of overlapped tiles (option tile_overlap; geometry in film_kernels.h).  No reference counterpart:
+// eval/interpolator.py:102-126 pastes non-overlapping tiles.  One thread owns four consecutive floats of an output row
+// and gathers them from the one, two (a ramp) or four (a corner) windows that cover them; 128-bit loads and stores
+// wherever the addresses allow.  Every output float is written once: no atomics, the same bits on every run.
+// ------------------------------------------------------------------------------------------
+// Windows ka, kb that coordinate x of an axis blends, and the weight t of kb.  ka == kb outside every ramp.
+__device__ __forceinline__ void stitch_sources(const StitchAxis& a, int x, int& ka, int& kb, float& t) {
+  const int k = x / a.p, r = x - k * a.p;
+  ka = kb = k;
+  t = 0.f;
+  if (k > 0 && r < a.v) {                        // ramp around c = k*p, upper half: x - (c - v) = r + v
+    ka = k - 1;
+    t = ((float)(r + a.v) + 0.5f) / (float)(2 * a.v);
+  } else if (k < a.b - 1 && r >= a.p - a.v) {    // ramp around c = (k+1)*p, lower half
+    kb = k + 1;
+    t = ((float)(r - (a.p - a.v)) + 0.5f) / (float)(2 * a.v);
+  }
+}
+
+__device__ __forceinline__ void stitch_load(const float* __restrict__ p, int n, float (&v)[4]) {
+  if (n == 4 && ((uintptr_t)p & 15) == 0) {
+    const float4 f = __ldg(reinterpret_cast<const float4*>(p));
+    v[0] = f.x, v[1] = f.y, v[2] = f.z, v[3] = f.w;
+  } else {
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      if (i < n) v[i] = __ldg(p + i);
+  }
+}
+
+// `n` floats of output row y from float column j on, all of whose pixels blend the same pair of window columns
+__device__ __forceinline__ void stitch_run(const float* __restrict__ tiles, int64_t tile_stride, const StitchGeom& g, int y,
+                                           int ya, int yb, float ty, int j, int n, float* __restrict__ o) {
+  int xa = 0, xb = 0;
+  float tx[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    if (i < n) stitch_sources(g.ax, (j + i) / 3, xa, xb, tx[i]);
+  auto src = [&](int ky, int kx) {
+    return tiles + (int64_t)g.slot[ky * g.ax.b + kx] * tile_stride +
+           ((int64_t)(y - stitch_origin(g.ay, ky)) * g.ax.q - stitch_origin(g.ax, kx)) * 3 + j;
+  };
+  // along W first, then along H; each blend is a lerp a + t * (b - a)
+  auto row = [&](int ky, float (&r)[4]) {
+    stitch_load(src(ky, xa), n, r);
+    if (xb != xa) {
+      float b[4];
+      stitch_load(src(ky, xb), n, b);
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+        if (i < n) r[i] = r[i] + tx[i] * (b[i] - r[i]);
+    }
+  };
+  float r[4];
+  row(ya, r);
+  if (yb != ya) {
+    float s[4];
+    row(yb, s);
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      if (i < n) r[i] = r[i] + ty * (s[i] - r[i]);
+  }
+  if (n == 4 && ((uintptr_t)o & 15) == 0) {
+    *reinterpret_cast<float4*>(o) = make_float4(r[0], r[1], r[2], r[3]);
+  } else {
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+      if (i < n) o[i] = r[i];
+  }
+}
+
+__global__ void __launch_bounds__(256) k_stitch_feather(const float* __restrict__ tiles, int64_t tile_stride,
+                                                        const __grid_constant__ StitchGeom g, float* __restrict__ out,
+                                                        int64_t out_pitch) {
+  const int row_floats = g.ax.L * 3;
+  const int j = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
+  const int y = blockIdx.y;
+  if (j >= row_floats) return;
+  const int n = min(4, row_floats - j);
+  int ya, yb, xa0, xb0, xa1, xb1;
+  float ty, t;
+  stitch_sources(g.ay, y, ya, yb, ty);
+  stitch_sources(g.ax, j / 3, xa0, xb0, t);
+  stitch_sources(g.ax, (j + n - 1) / 3, xa1, xb1, t);
+  float* o = out + (int64_t)y * out_pitch + j;
+  if (xa0 == xa1 && xb0 == xb1) {
+    stitch_run(tiles, tile_stride, g, y, ya, yb, ty, j, n, o);
+  } else {  // the four floats straddle the edge of a ramp: one float at a time
+    for (int i = 0; i < n; ++i) stitch_run(tiles, tile_stride, g, y, ya, yb, ty, j + i, 1, o + i);
+  }
+}
+
+cudaError_t launch_stitch_feather(const float* tiles, int64_t tile_stride, const StitchGeom& g, float* out,
+                                  int64_t out_pitch, cudaStream_t st) {
+  dim3 grid(cdiv((int64_t)g.ax.L * 3, 4 * 256), g.ay.L);
+  k_stitch_feather<<<grid, 256, 0, st>>>(tiles, tile_stride, g, out, out_pitch);
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------
 // feature_extractor.py:119  cfeat_conv_0: 3 -> 64, 3x3 SAME + bias + LeakyReLU, fp32 math.
 // 8 threads per pixel (8 output channels each); 32 pixels per 256-thread block.
 // ------------------------------------------------------------------------------------------

@@ -79,6 +79,29 @@ cudaError_t launch_pad_image(const float* src, int64_t src_pitch, int h, int w, 
 cudaError_t launch_u8_to_f32(const uint8_t* src, float* dst, int64_t n, cudaStream_t st);
 cudaError_t launch_f32_to_u8(const float* src, uint8_t* dst, int64_t n, cudaStream_t st);
 
+// Overlapped tiling (option tile_overlap).  One frame axis of length L = b * p cut into b windows of one length
+// q = p + 2v: window k starts at clamp(k*p - v, 0, L - q), so border windows are shifted inward, not shortened.
+// An axis with b == 1 has v = 0 (one window, nothing to blend).  0 <= 2v <= p keeps the ramps of consecutive
+// boundaries apart: a pixel sees at most two windows per axis.
+struct StitchAxis {
+  int b, p, v, q, L;
+};
+__host__ __device__ inline int stitch_origin(const StitchAxis& a, int k) {  // first coordinate of window k
+  const int o = k * a.p - a.v;
+  return o < 0 ? 0 : (o > a.L - a.q ? a.L - a.q : o);
+}
+constexpr int kMaxStitchTiles = 64;
+struct StitchGeom {
+  StitchAxis ay, ax;            // rows, columns
+  int slot[kMaxStitchTiles];    // tile t = ty * ax.b + tx lives at tiles + slot[t] * tile_stride
+};
+// Feathered stitch of [tiles][q_h][q_w][3] fp32 window results into an (H, W, 3) frame with row pitch `out_pitch`
+// floats.  Across the boundary c = k*p between windows k-1 (value a) and k (value b), for x in [c - v, c + v):
+// t = (x + 0.5 - (c - v)) / 2v, out = a + t * (b - a); elsewhere the pixel of the window whose core holds it.  Along W
+// first, then along H.  Gather form: every output float is written once, from at most four windows.
+cudaError_t launch_stitch_feather(const float* tiles, int64_t tile_stride, const StitchGeom& g, float* out,
+                                  int64_t out_pitch, cudaStream_t st);
+
 // debug: split tensor slice -> fp32 NHWC
 cudaError_t launch_unsplit(const sp_t* hi, const sp_t* lo, int C, int c_off, int Cn, int64_t npix,
                            float* out, cudaStream_t st);

@@ -196,6 +196,22 @@ class Interpolator:
                                                C.c_void_p(d_out), out_pitch, C.c_void_p(stream))
         self._check(st)
 
+    def stitch_tiles_device(self, d_tiles: int, tile_stride: int, height: int, width: int, block_shape: List[int],
+                            overlap: int, d_out: int, slot_of_tile: Optional[List[int]] = None,
+                            out_pitch: Optional[int] = None, stream: int = 0) -> None:
+        """Feathered stitch of overlapped window results on the device (film_stitch_tiles_device; geometry in
+        `spec.tile_windows`); asynchronous. Tile t is read at d_tiles + slot_of_tile[t] * tile_stride floats (identity
+        if None); the (height, width, 3) frame is written at d_out with row pitch `out_pitch` floats."""
+        bh, bw = int(block_shape[0]), int(block_shape[1])
+        slots = None
+        if slot_of_tile is not None:
+            assert len(slot_of_tile) == bh * bw, "slot_of_tile needs one entry per tile"
+            slots = (C.c_int * (bh * bw))(*[int(s) for s in slot_of_tile])
+        st = self._lib.film_stitch_tiles_device(self._handle, C.c_void_p(d_tiles), int(tile_stride), slots, int(height),
+                                                int(width), bh, bw, int(overlap), C.c_void_p(d_out),
+                                                int(out_pitch or width * 3), C.c_void_p(stream))
+        self._check(st)
+
     def interpolate_recursively(self, frame0: np.ndarray, frame1: np.ndarray,
                                 times_to_interpolate: int) -> np.ndarray:
         """All frames between two (H, W, 3) frames, end points included, in display order:

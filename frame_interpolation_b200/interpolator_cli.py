@@ -1,7 +1,7 @@
 """Command line front end with the reference's flags (eval/interpolator_cli.py:85-121) on the H100 engine.
 
     python -m frame_interpolation_b200.interpolator_cli --pattern "photos" --model_path synthetic \
-        --times_to_interpolate 3 [--align 64] [--block_height 2 --block_width 2] [--output_video --fps 30]
+        --times_to_interpolate 3 [--align 64] [--block_height 2 --block_width 2 [--tile_overlap 32]] [--output_video --fps 30]
 
 For every directory matching --pattern: the *.png/*.jpg/*.jpeg frames (natural order) are
 interpolated recursively and written to <dir>/interpolated_frames/frame_%03d.png
@@ -40,6 +40,10 @@ def build_parser() -> argparse.ArgumentParser:
     p.add_argument("--any_size", action="store_true",
                    help="Accept padded frame sizes that are not multiples of 64 (e.g. --align 0 at 1920x1080), like the "
                         "reference graph; off by default.")
+    p.add_argument("--tile_overlap", type=int, default=0,
+                   help="With --block_height/--block_width: interpolate every tile on a window this many pixels larger on "
+                        "each interior side and cross-fade neighbouring tiles over twice that width, instead of pasting "
+                        "non-overlapping tiles like the reference (0, the default).")
     p.add_argument("--output_video", action="store_true")
     p.add_argument("--device", type=int, default=None, help="CUDA device ordinal (default: LOCAL_RANK or 0)")
     return p
@@ -110,6 +114,8 @@ def main(argv=None) -> int:
     interpolator = Interpolator(args.model_path, args.align, [args.block_height, args.block_width], device=device)
     if args.any_size:
         interpolator.set_option("any_size", 1)
+    if args.tile_overlap:
+        interpolator.set_option("tile_overlap", args.tile_overlap)
     for d in mine:
         n = process_directory(d, interpolator, args.times_to_interpolate, args.fps, args.output_video)
         print(f"[film_b200] {d}: wrote {n} frames to {d}/interpolated_frames", flush=True)

@@ -9,6 +9,8 @@ The path shards into independent units:
   tiles (eval/interpolator.py:192-206) are independent by construction (no halo, each
   tile padded on its own), so tile t goes to rank t % world; ONE all-gather reassembles
   the stitched frame (NCCL over NVLink on GPUs; gloo on CPU for the host-logic tests).
+  With `overlap` > 0 every tile runs on its window of `spec.tile_windows` and the gathered
+  results are cross-faded instead of pasted (engine option tile_overlap).
 * recursion    -- `interpolate_recursively`: eval/util.py:62-91's binary dependency tree
   scheduled level-synchronously: the 2^(k-1) calls of level k are sharded, new mid-frames
   are all-gathered so every rank holds the parents of level k+1; the output order is the
@@ -23,6 +25,8 @@ from __future__ import annotations
 from typing import Callable, List, Optional, Sequence, Tuple
 
 import numpy as np
+
+from . import spec
 
 Engine = Callable[[np.ndarray, np.ndarray, np.ndarray], np.ndarray]
 
@@ -88,14 +92,20 @@ def interpolate_pairs(engine: Engine, x0: np.ndarray, x1: np.ndarray, device=Non
 
 
 def interpolate_tiled(engine: Engine, x0: np.ndarray, x1: np.ndarray, block_shape: Sequence[int],
-                      device=None, group=None) -> np.ndarray:
+                      device=None, group=None, overlap: int = 0) -> np.ndarray:
     """The reference's tiled path with tiles sharded round-robin over ranks and one
-    all-gather to reassemble (eval/interpolator.py:192-206 runs them sequentially)."""
+    all-gather to reassemble (eval/interpolator.py:192-206 runs them sequentially).
+    overlap > 0: every tile runs on its window of `spec.tile_windows` and the results are cross-faded
+    (`spec.stitch_overlapped`, rounded to float32) instead of pasted."""
     from .interpolator import image_to_patches, patches_to_image
     world, rank = _world_rank(group)
     bh, bw = int(block_shape[0]), int(block_shape[1])
-    p0 = image_to_patches(x0, [bh, bw])
-    p1 = image_to_patches(x1, [bh, bw])
+    if overlap:
+        origins, (qh, qw) = spec.tile_windows(x0.shape[1], x0.shape[2], [bh, bw], overlap)
+        p0, p1 = (np.stack([x[0, y:y + qh, c:c + qw] for y, c in origins]) for x in (x0, x1))
+    else:
+        p0 = image_to_patches(x0, [bh, bw])
+        p1 = image_to_patches(x1, [bh, bw])
     nt = bh * bw
     mine = round_robin(nt, world, rank)
     dt = np.full((1,), 0.5, np.float32)
@@ -110,6 +120,8 @@ def interpolate_tiled(engine: Engine, x0: np.ndarray, x1: np.ndarray, block_shap
         tiles[order] = gathered
     else:
         tiles = local
+    if overlap:
+        return spec.stitch_overlapped(tiles, x0.shape[1], x0.shape[2], [bh, bw], overlap).astype(np.float32)
     return patches_to_image(tiles, [bh, bw])
 
 
@@ -171,7 +183,37 @@ def device_engine(interp):
         cur.wait_stream(es)
         for t in (x0, x1, out):
             t.record_stream(es)
+
+    def stitch(tiles, slot_of_tile, block_shape, overlap, out):
+        """Feathered stitch (film_stitch_tiles_device) of the window results in `tiles` (slots, q_h, q_w, 3), tile t in
+        slot slot_of_tile[t], into the (H, W, 3) view `out`; same stream semantics as the network call."""
+        h, w, _ = out.shape
+        qh, qw = tiles.shape[-3], tiles.shape[-2]
+        assert tiles.dtype == out.dtype == torch.float32 and tiles.is_cuda and tiles.is_contiguous()
+        assert (qh, qw) == spec.tile_windows(h, w, block_shape, overlap)[1], "tiles do not have the window shape"
+        assert max(slot_of_tile) < tiles.numel() // (qh * qw * 3), "slot outside the tile buffer"
+        assert out.stride(2) == 1 and out.stride(1) == 3, "inner dims must be dense (row-pitched view)"
+        dev = out.device
+        if dev not in side:
+            side[dev] = torch.cuda.Stream(device=dev)
+        es, cur = side[dev], torch.cuda.current_stream(dev)
+        es.wait_stream(cur)
+        interp.stitch_tiles_device(tiles.data_ptr(), qh * qw * 3, h, w, block_shape, overlap, out.data_ptr(),
+                                   slot_of_tile=slot_of_tile, out_pitch=out.stride(0), stream=es.cuda_stream)
+        cur.wait_stream(es)
+        for t in (tiles, out):
+            t.record_stream(es)
+    run.stitch = stitch
     return run
+
+
+def stitch_tiles_host(tiles, slot_of_tile, block_shape, overlap, out):
+    """The `stitch` of a CPU stand-in for `device_engine` (host-logic tests): `spec.stitch_overlapped` on CPU tensors."""
+    import torch
+    qh, qw = tiles.shape[-3], tiles.shape[-2]
+    t = tiles.reshape(-1, qh, qw, 3)[list(slot_of_tile)].numpy()
+    res = spec.stitch_overlapped(t, out.shape[0], out.shape[1], block_shape, overlap)[0]
+    out.copy_(torch.from_numpy(res.astype(np.float32)))
 
 
 def _all_gather_slots(buf, group=None):
@@ -185,39 +227,49 @@ def _all_gather_slots(buf, group=None):
     return buf
 
 
+def window_view(frame, block_shape, t, overlap):
+    """Window of tile t (row-major; `spec.tile_windows`) of a (1, H, W, 3) or (H, W, 3) tensor as a strided view."""
+    f = frame[0] if frame.dim() == 4 else frame
+    origins, (qh, qw) = spec.tile_windows(f.shape[0], f.shape[1], block_shape, overlap)
+    y, x = origins[t]
+    return f[y:y + qh, x:x + qw]
+
+
 def tile_view(frame, block_shape, t):
     """Tile t (row-major, eval/interpolator.py:66-99) of a (1, H, W, 3) or (H, W, 3) tensor as a strided view."""
-    f = frame[0] if frame.dim() == 4 else frame
-    bh, bw = int(block_shape[0]), int(block_shape[1])
-    h, w = f.shape[0], f.shape[1]
-    assert h % bh == 0, 'block_height=%d should evenly divide height=%d.' % (bh, h)
-    assert w % bw == 0, 'block_width=%d should evenly divide width=%d.' % (bw, w)
-    ph, pw = h // bh, w // bw
-    r, c = divmod(t, bw)
-    return f[r * ph:(r + 1) * ph, c * pw:(c + 1) * pw]
+    return window_view(frame, block_shape, t, 0)
 
 
-def interpolate_tiled_device(engine_dev, x0, x1, block_shape, group=None, out=None, gather_buf=None):
+def interpolate_tiled_device(engine_dev, x0, x1, block_shape, group=None, out=None, gather_buf=None, overlap=0):
     """Tiled path with tiles sharded round-robin over ranks, device-resident end to end.
 
     x0, x1: (1, H, W, 3) tensors resident on every rank's device. Rank r computes tiles
     r, r + world, ... and the network writes each of them directly into slot [r, j] of the
     all-gather buffer; ONE NCCL all-gather; one device copy stitches the rank-major slots
-    into the (1, H, W, 3) frame (`out`, allocated if None). Returns `out`."""
+    into the (1, H, W, 3) frame (`out`, allocated if None). Returns `out`.
+
+    overlap > 0: the slots have the window shape of `spec.tile_windows`, every tile runs on its window, and
+    `engine_dev.stitch` (the feathered stitch kernel behind `device_engine`; `stitch_tiles_host` for a CPU stand-in)
+    reads the rank-major slots in place through a slot table."""
     import torch
     world, rank = _world_rank(group)
     bh, bw = int(block_shape[0]), int(block_shape[1])
     nt = bh * bw
     _, h, w, _ = x0.shape
-    ph, pw = h // bh, w // bw
+    ph, pw = spec.tile_windows(h, w, [bh, bw], overlap)[1]
     m = (nt + world - 1) // world
     if gather_buf is None:
         gather_buf = torch.empty((world, m, ph, pw, 3), dtype=torch.float32, device=x0.device)
     for j, t in enumerate(round_robin(nt, world, rank)):
-        engine_dev(tile_view(x0, block_shape, t), tile_view(x1, block_shape, t), gather_buf[rank, j])
+        engine_dev(window_view(x0, block_shape, t, overlap), window_view(x1, block_shape, t, overlap), gather_buf[rank, j])
     _all_gather_slots(gather_buf, group)
     if out is None:
         out = torch.empty((1, h, w, 3), dtype=torch.float32, device=x0.device)
+    if overlap:
+        # slot [r, j] holds tile j * world + r
+        engine_dev.stitch(gather_buf.view(world * m, ph, pw, 3), [(t % world) * m + t // world for t in range(nt)],
+                          [bh, bw], overlap, out[0])
+        return out
     # slot [r, j] holds tile j * world + r -> tile-major order, then patches_to_image as one strided copy
     tiles = gather_buf.transpose(0, 1).reshape(world * m, ph, pw, 3)[:nt]
     out.view(bh, ph, bw, pw, 3).copy_(tiles.view(bh, bw, ph, pw, 3).permute(0, 2, 1, 3, 4))

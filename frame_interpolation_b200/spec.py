@@ -12,7 +12,9 @@ file is validated against them at load time.
 """
 from __future__ import annotations
 
-from typing import Dict, List, Tuple
+from typing import Dict, List, Sequence, Tuple
+
+import numpy as np
 
 PYRAMID_LEVELS = 7
 FUSION_PYRAMID_LEVELS = 5
@@ -132,3 +134,66 @@ def padded_shape(h: int, w: int, align: int | None) -> Tuple[int, int, int, int]
     ph = (align - h % align) if h % align else 0
     pw = (align - w % align) if w % align else 0
     return h + ph, w + pw, ph // 2, pw // 2
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Overlapped tiling (engine option tile_overlap; no reference counterpart: eval/interpolator.py:66-126 cuts and pastes
+# non-overlapping tiles).  One rule per axis, the same along H and W; csrc/film_engine.cu (stitch_axis) and
+# csrc/film_kernels.cu (k_stitch_feather) restate it.
+# ---------------------------------------------------------------------------------------------------------------------
+def _axis_windows(length: int, blocks: int, overlap: int, name: str) -> Tuple[List[int], int, int]:
+    """-> (window origins, window length q, effective overlap v) of one frame axis of `length` in `blocks` blocks."""
+    p = length // blocks
+    assert length == p * blocks, 'block_%s=%d should evenly divide %s=%d.' % (name, blocks, name, length)
+    v = int(overlap) if blocks > 1 else 0          # a single block has no boundary to blend across
+    assert v >= 0, 'tile overlap must not be negative'
+    # keeps the ramps of consecutive boundaries apart: no pixel sees more than two windows per axis
+    assert 2 * v <= p, 'tile_overlap=%d is more than half the tile %s=%d.' % (v, name, p)
+    q = p + 2 * v
+    # every window has the length q: border windows are shifted inward, not shortened, so a frame needs one plan
+    return [min(max(k * p - v, 0), length - q) for k in range(blocks)], q, v
+
+
+def tile_windows(h: int, w: int, block_shape: Sequence[int], overlap: int) -> Tuple[List[Tuple[int, int]], Tuple[int, int]]:
+    """Windows of an h x w frame cut into block_shape = [bh, bw] tiles that reach `overlap` pixels past every interior
+    tile boundary: (origins, (q_h, q_w)) with origins[t] = (y, x) of tile t (row-major) and one shape for all windows.
+    overlap = 0 gives the reference's tiles (eval/interpolator.py:66-99)."""
+    bh, bw = int(block_shape[0]), int(block_shape[1])
+    oy, qh, _ = _axis_windows(h, bh, overlap, "height")
+    ox, qw, _ = _axis_windows(w, bw, overlap, "width")
+    return [(y, x) for y in oy for x in ox], (qh, qw)
+
+
+def _axis_blend(length: int, blocks: int, overlap: int, name: str):
+    """Per coordinate x of the axis: the two windows (ka, kb) it blends, the weight t of kb, and its coordinate inside
+    each of them.  At the boundary c = k*p, for x in [c - v, c + v): t = (x + 0.5 - (c - v)) / 2v between windows k-1
+    and k; elsewhere ka == kb == the window whose core contains x."""
+    origins, _, v = _axis_windows(length, blocks, overlap, name)
+    p = length // blocks
+    x = np.arange(length)
+    k = x // p
+    ka, kb, t = k.copy(), k.copy(), np.zeros(length, np.float64)
+    for c in range(p, length, p) if v else ():
+        ramp = (x >= c - v) & (x < c + v)
+        ka[ramp], kb[ramp] = c // p - 1, c // p
+        t[ramp] = (x[ramp] + 0.5 - (c - v)) / (2 * v)
+    o = np.asarray(origins)
+    return ka, kb, t, x - o[ka], x - o[kb]
+
+
+def stitch_overlapped(tiles: np.ndarray, h: int, w: int, block_shape: Sequence[int], overlap: int) -> np.ndarray:
+    """Feathered stitch of the (bh*bw, q_h, q_w, C) window results of `tile_windows` into a (1, h, w, C) float64 frame:
+    out = a + t * (b - a) across every interior boundary, along W first, then along H.  The numpy statement of what
+    the engine's k_stitch_feather computes in float32."""
+    bh, bw = int(block_shape[0]), int(block_shape[1])
+    _, (qh, qw) = tile_windows(h, w, block_shape, overlap)
+    t = np.asarray(tiles, np.float64)
+    assert t.shape[:3] == (bh * bw, qh, qw), "expected %d windows of %dx%d" % (bh * bw, qh, qw)
+    t = t.reshape(bh, bw, qh, qw, -1)
+    xa, xb, tx, ia, ib = _axis_blend(w, bw, overlap, "width")
+    ya, yb, ty, ja, jb = _axis_blend(h, bh, overlap, "height")
+    a, b = t[:, xa, :, ia], t[:, xb, :, ib]                  # (w, bh, q_h, C): every tile row blended along W
+    rows = a + tx[:, None, None, None] * (b - a)
+    a, b = rows[:, ya, ja], rows[:, yb, jb]                  # (w, h, C)
+    out = a + ty[None, :, None] * (b - a)
+    return np.ascontiguousarray(out.transpose(1, 0, 2))[np.newaxis]

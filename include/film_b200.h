@@ -93,7 +93,12 @@ FILM_API int film_interpolate(film_handle* h, const float* x0, const float* x1, 
 
 /* Host pointers, B == 1. Splits the frame into block_h x block_w non-overlapping tiles
  * (row-major tile order), pads every tile independently to `align`, runs the network
- * per tile, stitches. H % block_h == 0 and W % block_w == 0 or status 1. */
+ * per tile, stitches. H % block_h == 0 and W % block_w == 0 or status 1.
+ * With the option "tile_overlap" = v > 0 (no reference counterpart) every tile runs on a window that reaches v pixels
+ * past each interior tile boundary and neighbouring results are cross-faded over the 2v pixels around the boundary:
+ * both frames are uploaded once, the windows run as views of the resident frames, film_stitch_tiles_device blends them,
+ * one download.  2v must not exceed the tile height (block_h > 1) or width (block_w > 1), else status 1; at most 64
+ * tiles.  film_profile then reports the padded window size. */
 FILM_API int film_interpolate_tiled(film_handle* h, const float* x0, const float* x1, const float* dt,
                            int H, int W, int align, int block_h, int block_w, float* out);
 
@@ -104,6 +109,22 @@ FILM_API int film_interpolate_tiled(film_handle* h, const float* x0, const float
 FILM_API int film_interpolate_device(film_handle* h, const float* d_x0, const float* d_x1,
                             int B, int H, int W, int64_t in_pitch, int align,
                             float* d_out, int64_t out_pitch, void* cuda_stream);
+
+/* Feathered stitch of overlapped tiles, device pointers, asynchronous on `cuda_stream` like film_interpolate_device.
+ * Geometry, the same along H and W: a frame axis of length L in b blocks has the core length p = L / b.  b == 1: one
+ * window [0, L), nothing is blended.  b > 1: every window has the length q = p + 2 * overlap and window k starts at
+ * clamp(k*p - overlap, 0, L - q): border windows are shifted inward, not shortened, so all block_h * block_w windows of
+ * a frame have one shape (q_h, q_w).  Tile t (row-major) is read as [q_h][q_w][3] floats at
+ * d_tiles + slot_of_tile[t] * tile_stride (tile_stride in floats, >= q_h*q_w*3; slot_of_tile: HOST array of
+ * block_h*block_w ints read before the call returns, NULL = identity; a rank-major all-gather buffer is read in place
+ * through it).  At the boundary c = k*p between tiles k-1 (value a) and k (value b), for x in [c - overlap, c + overlap):
+ * t = (x + 0.5 - (c - overlap)) / (2 * overlap), out = a + t * (b - a); every other pixel comes from the tile whose core
+ * contains it; along W first, then along H.  Every output float is written once (no atomics: results are
+ * run-to-run identical) through the row pitch out_pitch (floats, >= W*3).  Status 1 unless 0 <= 2 * overlap <= p on
+ * every axis with b > 1, block_h * block_w <= 64 and H <= 65535. */
+FILM_API int film_stitch_tiles_device(film_handle* h, const float* d_tiles, int64_t tile_stride, const int* slot_of_tile,
+                                      int H, int W, int block_h, int block_w, int overlap, float* d_out,
+                                      int64_t out_pitch, void* cuda_stream);
 
 /* Recursive mid-point interpolation between two (H, W, 3) host frames, the whole binary tree of
  * eval/util.py:62-91 (`_recursive_generator`) evaluated with every intermediate frame resident in
@@ -171,6 +192,11 @@ FILM_API int film_profile(film_handle* h, film_profile_t* out);
  *                   fail with status 1): pyramid levels floor like its VALID pooling, and a decoder level that is not
  *                   exactly twice the coarser one gets a nearest resize of its own before fusion conv_0.  Only decides
  *                   whether a size is accepted: a 64-aligned size runs the same plan either way
+ *   "tile_overlap": film_interpolate_tiled only.  0 = the reference's tiling: non-overlapping tiles, pasted (default),
+ *                   v > 0 = every tile is interpolated on a window v pixels larger on each interior side and neighbouring
+ *                   results are cross-faded over 2v pixels (see film_stitch_tiles_device); negative values are stored
+ *                   as 0.  The output then differs from the reference's, which is why it is never chosen for the caller.
+ *                   Not a plan key: the window shape selects the plan, and one frame needs one plan
  *   "use_lanes"   : 1 = enqueue independent branches on separate streams (default 0)
  *   "clear_plans" : (any value) drop every cached (H, W, align) plan -- CUDA graph and activation arena --
  *                   after draining the handle's stream.  Plans are cached per shape and never evicted
