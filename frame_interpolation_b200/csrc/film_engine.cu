@@ -80,7 +80,7 @@ constexpr uint32_t kDefaultOnepassMask =
 struct Options {
   int conv_impl = 0;     // 0 = tensor-core kernels, 1 = fp32 CUDA-core validation kernels
   int use_graph = 1;     // capture each plan's schedule in a CUDA graph
-  int keep_debug = 0;    // keep every intermediate readable (no arena reuse, no fused RGB head)
+  int keep_debug = 0;    // keep every intermediate readable: turns arena reuse off and nothing else, so the same kernels run
   int time_ops = 0;      // eager runs with one CUDA-event pair per op (film_op_table)
   int use_lanes = 0;     // stream lanes: measured no gain at 1080p (smem-saturating kernels cannot co-reside)
   int conv3x3_v2 = 1;    // persistent tap-reuse kernel for 3x3 convs
@@ -573,7 +573,8 @@ struct Plan {
     int lane;                  // stream lane the op is enqueued on
     std::vector<int> waits;    // tokens (events) the op waits for before it starts
     std::vector<int> signals;  // tokens recorded after the op
-    std::string form = "";     // conv kernel form: "3x3", "3x3_pxn" (persistent kernel), "tc" (generic), "simt"
+    std::string form = "";     // conv kernel form: "3x3", "3x3_pxn", "3x3_pair" (persistent kernel), "tc" (generic), "simt"
+    int passes = 0;            // tensor-core passes of a conv: 1 (hi x hi) or 3 (split product); 0 for other ops
   };
   std::vector<Op> ops;
   std::vector<float> op_ms;  // filled by timed eager runs
@@ -849,6 +850,11 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
     alg_bytes += (double)pc.cout * ktot * 2.0 * planes_in;
   }
   P.last_conv_bytes = alg_bytes;
+  // debug hooks: the whole destination of the call site (all B batches, its cout real channels) and its fused pool
+  if (out && sy == 1 && sx == 1 && !tag.empty())
+    P.debug["out:" + tag] = DebugTensor{true, out->hi, out->lo, out->pixels(), out->C, out_c_off, pc.cout};
+  if (pool_out)
+    P.debug["pool:" + tag] = DebugTensor{true, pool_out->hi, pool_out->lo, pool_out->pixels(), pool_out->C, 0, pc.cout};
   if (no_op) return idx;  // the caller launches this problem as part of a group
   Plan* pp = &P;
   const int impl = o.conv_impl;
@@ -857,7 +863,8 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
     return v2 ? launch_conv3x3_tc(pp->d_probs + idx, pp->h_probs[idx], st)
               : launch_conv_tc(pp->d_probs + idx, pp->h_probs[idx], st);
   }, 2.0 * ref_macs_per_px * (double)cp.B * cp.H * cp.W, alg_bytes);
-  P.ops.back().form = impl == 1 ? "simt" : !v2 ? "tc" : cp.pxn ? "3x3_pxn" : "3x3";
+  P.ops.back().form = impl == 1 ? "simt" : !v2 ? "tc" : cp.pxn ? "3x3_pxn" : cp.pair ? "3x3_pair" : "3x3";
+  P.ops.back().passes = cp.passes;
   return idx;
 }
 
@@ -880,7 +887,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
   P.opt = opt;
   P.reuse = !opt.keep_debug && !opt.use_lanes && opt.arena_reuse;
   // the RGB head and the crop run in the epilogue of fusion_conv2@L0 instead of a kernel of their own
-  const bool fuse_rgb = opt.conv_impl == 0 && opt.conv3x3_v2 && opt.fuse_rgb_head && !opt.keep_debug;
+  const bool fuse_rgb = opt.conv_impl == 0 && opt.conv3x3_v2 && opt.fuse_rgb_head;
   P.h = h;
   P.w = w;
   P.num_sms = num_sms;
@@ -902,7 +909,10 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
 
   // ---- image pyramids (util.py:23-45), both images batched: img[l] = [2][H_l][W_l][3]
   float* img[kLevels];
-  for (int l = 0; l < kLevels; ++l) img[l] = P.alloc<float>((int64_t)2 * Hs[l] * Ws[l] * 3, true);
+  for (int l = 0; l < kLevels; ++l) {
+    img[l] = P.alloc<float>((int64_t)2 * Hs[l] * Ws[l] * 3, true);
+    P.debug["img/" + std::to_string(l)] = DebugTensor{false, img[l], nullptr, (int64_t)2 * Hs[l] * Ws[l], 3, 0, 3};
+  }
   for (int k = 0; k < 2; ++k) {
     float* dst = img[0] + (int64_t)k * P.H * P.W * 3;
     const float* src = P.xin + (int64_t)k * h * w * 3;
@@ -947,6 +957,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
         P.add_op(2, std::string(pool_dst ? "fe_conv0+pool@L" : "fe_conv0@L") + std::to_string(r),
                  [=](cudaStream_t st) { return launch_fe_conv0(im, 2, hh, ww, w0, b0, oh, ol, lo_skip, pool_dst, st); },
                  2.0 * 27 * 64 * 2.0 * hh * ww, 2.0 * hh * ww * (3 * 4 + 64 * (lo_skip ? 2.0 : 4.0)));
+        P.debug["out:" + P.ops.back().name] = DebugTensor{true, t1->hi, t1->lo, t1->pixels(), t1->C, 0, 64};
       } else if (j == 0 && opt.conv_impl == 0 && opt.conv3x3_v2) {
         // cfeat_conv_0 on the persistent 3x3 tensor-core kernel: the image is widened to a 32-channel
         // split tensor (3 real channels), K = 9 taps x one 32-channel block
@@ -956,6 +967,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
         P.add_op(2, "fe_split32@L" + std::to_string(r),
                  [=](cudaStream_t st) { return launch_image_to_split32(im, 2, hh, ww, im32->hi, im32->lo, st); }, 0,
                  2.0 * hh * ww * (12 + 32.0));
+        P.debug["out:" + P.ops.back().name] = DebugTensor{true, im32->hi, im32->lo, im32->pixels(), 32, 0, 32};
         add_conv(P, "fe_conv0@L" + std::to_string(r), 27.0 * 64, M.fe0_3x3, {{im32, 0}}, 1, t1, 0, fe_stage(i, 0), fe_stage(i, 1));
       } else if (j == 0 && opt.conv_impl == 0) {
         // generic-kernel variant: im2col-lite (27 -> 32 channels) + a 1x1 conv, K = 32
@@ -965,6 +977,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
         P.add_op(2, "fe_im2col@L" + std::to_string(r),
                  [=](cudaStream_t st) { return launch_im2col3x3(im, 2, hh, ww, col->hi, col->lo, st); }, 0,
                  2.0 * hh * ww * (12 + 128.0));
+        P.debug["out:" + P.ops.back().name] = DebugTensor{true, col->hi, col->lo, col->pixels(), 32, 0, 32};
         add_conv(P, "fe_conv0@L" + std::to_string(r), 27.0 * 64, M.fe[0], {{col, 0}}, 1, t1, 0, fe_stage(i, 0), fe_stage(i, 1));
       } else if (j == 0) {
         const float* im = img[i];
@@ -974,6 +987,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
         P.add_op(2, "fe_conv0@L" + std::to_string(r),
                  [=](cudaStream_t st) { return launch_conv0_c3(im, 2, hh, ww, w0, b0, oh, ol, 64, 0, st); },
                  2.0 * 27 * 64 * 2.0 * hh * ww, 2.0 * hh * ww * (3 + 64) * 4.0);
+        P.debug["out:" + P.ops.back().name] = DebugTensor{true, t1->hi, t1->lo, t1->pixels(), t1->C, 0, 64};
       } else {
         add_conv(P, "fe_conv" + std::to_string(2 * j) + "@L" + std::to_string(r), 9.0 * (c / 2) * c, M.fe[2 * j],
                  {{pooled, 0}}, 1, t1, 0, fe_stage(i, 2 * j), fe_stage(i, 2 * j + 1));
@@ -1000,6 +1014,9 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
         P.add_op(2, "fe_pool@L" + std::to_string(r), [=](cudaStream_t st) {
           return launch_act_pool(f->hi, f->lo, f->C, so, 2, f->H, f->W, c, po->hi, po->lo, po->C, st);
         });
+        // the same name as a fused pool: fe_pool@L<r> is not unique (every sub-tree that reaches level r pools there)
+        P.debug["pool:fe_conv" + std::to_string(2 * j + 1) + "@L" + std::to_string(r)] =
+            DebugTensor{true, po->hi, po->lo, po->pixels(), po->C, 0, c};
       }
     }
   }
@@ -1200,6 +1217,10 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
         }
         return cudaSuccess;
       }, 0, rbytes);
+      for (size_t k = 0; k < jobs.size(); ++k) {   // the resized coarse level (B = 2 warped batches), then its side tensor
+        const SplitBuf* d = jobs[k].second;
+        P.debug["out:" + P.ops.back().name + (k ? ":side" : "")] = DebugTensor{true, d->hi, d->lo, d->pixels(), d->C, 0, d->C};
+      }
       add_conv(P, "fusion_up@L" + std::to_string(i), 4.0 * M.fus_up_2x2[i].cin_ref * nf, M.fus_up_2x2[i], up_src, 0, up, 0,
                ST_FUS + 3 * i, ST_FUS + 3 * i + 1);
       for (auto& j : jobs) P.release(j.second);   // read by that conv only
@@ -1219,6 +1240,8 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
       P.add_op(0, "fusion_up@L" + std::to_string(i), [pq, first](cudaStream_t st) {
         return launch_conv_tc(pq->d_probs + first, pq->h_probs[first], st);
       }, fl, up_bytes);
+      P.ops.back().form = "tc";
+      P.ops.back().passes = P.h_probs[first].passes;
     } else {
       for (int py = 0; py < 2; ++py)
         for (int px = 0; px < 2; ++px)
@@ -1226,6 +1249,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
                    4.0 * M.fus_up[i][0].cin_ref * nf, M.fus_up[i][py * 2 + px], up_src, 0, up, 0, ST_FUS + 3 * i,
                    ST_FUS + 3 * i + 1, 2, 2, py, px);
     }
+    P.debug["out:fusion_up@L" + std::to_string(i)] = DebugTensor{true, up->hi, up->lo, up->pixels(), up->C, 0, nf};
     SplitBuf* f1 = P.split(1, hh, ww, cpad);
     SplitBuf* f2 = (fuse_rgb && i == 0) ? nullptr : P.split(1, hh, ww, cpad);
     add_conv(P, "fusion_conv1@L" + std::to_string(i), 9.0 * M.fus_c1[i].cin_ref * nf, M.fus_c1[i],
@@ -2104,12 +2128,14 @@ int film_profile(film_handle* h, film_profile_t* out) {
 int film_op_table(film_handle* h, char* buf, int64_t buf_size, int64_t* needed) {
   if (!h || !h->last_plan) return FILM_ERR_ARG;
   try {
-  std::string out = "idx,category,name,ms,ref_flops,alg_bytes,form\n";
+  std::string out = "idx,category,name,ms,ref_flops,alg_bytes,form,passes\n";
   Plan* P = h->last_plan;
   for (size_t i = 0; i < P->ops.size(); ++i) {
     char line[256];
-    snprintf(line, sizeof(line), "%zu,%d,%s,%.6f,%.0f,%.0f,%s\n", i, P->ops[i].category, P->ops[i].name.c_str(),
-             i < P->op_ms.size() ? P->op_ms[i] : -1.f, P->ops[i].flops, P->ops[i].bytes, P->ops[i].form.c_str());
+    const std::string passes = P->ops[i].passes ? std::to_string(P->ops[i].passes) : "";
+    snprintf(line, sizeof(line), "%zu,%d,%s,%.6f,%.0f,%.0f,%s,%s\n", i, P->ops[i].category, P->ops[i].name.c_str(),
+             i < P->op_ms.size() ? P->op_ms[i] : -1.f, P->ops[i].flops, P->ops[i].bytes, P->ops[i].form.c_str(),
+             passes.c_str());
     out += line;
   }
   if (needed) *needed = (int64_t)out.size() + 1;
@@ -2127,18 +2153,32 @@ int film_debug_read(film_handle* h, const char* name, float* dst, int64_t* count
   if (!h || !name) return FILM_ERR_ARG;
   try {
     if (!h->last_plan) throw Error{FILM_ERR_ARG, "no call has been made yet"};
-    auto it = h->last_plan->debug.find(name);
+    // "<tensor>.hi" / "<tensor>.lo": one 16-bit plane of a split tensor, widened to float32
+    std::string base(name);
+    int plane = -1;
+    const size_t n_base = base.size();
+    if (n_base > 3 && (base.compare(n_base - 3, 3, ".hi") == 0 || base.compare(n_base - 3, 3, ".lo") == 0)) {
+      plane = base[n_base - 2] == 'h' ? 0 : 1;
+      base.resize(n_base - 3);
+    }
+    auto it = h->last_plan->debug.find(base);
     if (it == h->last_plan->debug.end()) throw Error{FILM_ERR_ARG, std::string("unknown debug tensor ") + name};
     const DebugTensor& d = it->second;
     if (d.recycled)
       throw Error{FILM_ERR_ARG, std::string(name) + " lives in a recycled activation buffer: set option keep_debug = 1 "
                                                     "before the call to read intermediates"};
+    if (plane >= 0 && !d.split) throw Error{FILM_ERR_ARG, base + " is a float32 tensor: it has no planes"};
     const int64_t n = d.npix * d.Cn;
     if (count) *count = n;
     if (!dst) return FILM_OK;
     FILM_CUDA(cudaSetDevice(h->device));
     FILM_CUDA(cudaStreamSynchronize(h->stream));
-    if (!d.split) {
+    if (plane >= 0) {
+      std::vector<uint16_t> raw((size_t)d.npix * d.C);   // every channel, then the slice on the host
+      FILM_CUDA(cudaMemcpy(raw.data(), plane ? d.p1 : d.p0, raw.size() * 2, cudaMemcpyDeviceToHost));
+      for (int64_t px = 0; px < d.npix; ++px)
+        for (int c = 0; c < d.Cn; ++c) dst[px * d.Cn + c] = sp_to_f32(raw[(size_t)px * d.C + d.c_off + c]);
+    } else if (!d.split) {
       FILM_CUDA(cudaMemcpy(dst, d.p0, n * 4, cudaMemcpyDeviceToHost));
     } else {
       float* tmp;

@@ -317,7 +317,8 @@ class Interpolator:
         for r in rows[1:]:
             v = r.split(",")
             out.append({"idx": int(v[0]), "category": int(v[1]), "name": v[2], "ms": float(v[3]),
-                        "ref_flops": float(v[4]), "alg_bytes": float(v[5]), "form": v[6]})
+                        "ref_flops": float(v[4]), "alg_bytes": float(v[5]), "form": v[6],
+                        "passes": int(v[7]) if v[7] else None})
         return out
 
     @property

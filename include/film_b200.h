@@ -162,7 +162,8 @@ FILM_API int film_profile(film_handle* h, film_profile_t* out);
  *                       tests to cross-check the tensor-core path on the device)
  *   "use_graph"   : 1 = capture each shape's schedule in a CUDA graph (default), 0 = eager
  *   "keep_debug"  : 1 = keep every intermediate tensor alive (no arena reuse) so that film_debug_read can
- *                   return it after the call; 0 (default) = activation buffers are recycled inside a plan
+ *                   return it after the call; it changes nothing else, so the same kernels run and the output is
+ *                   bit-identical; 0 (default) = activation buffers are recycled inside a plan
  *   "time_ops"    : 1 = run eagerly with one CUDA-event pair per kernel (see film_op_table)
  *   "conv3x3_v2"  : 1 = persistent tap-reuse kernel for 3x3 convs (default), 0 = generic kernel
  *   "conv3x3_2cta": 1 = the streamed-weight 3x3 convs of the large pyramid levels run as (2,1,1) CTA clusters in which
@@ -218,13 +219,21 @@ FILM_API int film_stage_name(int stage, char* buf, int buf_size);
 
 /* Debug/parity hook: copies an intermediate tensor of the LAST call to host as float32
  * NHWC. `name` is e.g. "feat0/3" (feature pyramid of image 0, level 3), "flow_fwd/0",
- * "flow_bwd/2", "image". Returns the element count through *count when dst == NULL. */
+ * "flow_bwd/2", "image", "img/2" (image pyramid level, [2][H_l][W_l][3]).  The destination of
+ * every conv op of film_op_table is "out:<op name>" (its cout real channels over all batches;
+ * the pooled output of a conv, fused or by fe_pool@L<r>: "pool:<conv op name>"), and so are the
+ * outputs of fe_conv0*, fe_split32@L*, fe_im2col@L* and fusion_resize@L* (that one's resized side
+ * tensor: "out:fusion_resize@L<i>:side").  "fusion_net/0" is absent when the RGB head is fused.
+ * "<name>.hi" / "<name>.lo" return one 16-bit plane of a split tensor as float32 (a plane that
+ * was never written reads as zeros).  Returns the element count through *count when dst == NULL. */
 FILM_API int film_debug_read(film_handle* h, const char* name, float* dst, int64_t* count);
 
 /* Per-op table of the plan used by the last call, as CSV text
- * "idx,category,name,ms,ref_flops,alg_bytes,form" (category 0 = tensor-core conv, 1 = warp gather,
+ * "idx,category,name,ms,ref_flops,alg_bytes,form,passes" (category 0 = tensor-core conv, 1 = warp gather,
  * 2 = other bandwidth kernels; form = the kernel of a conv: "3x3" / "3x3_pxn" persistent 3x3 kernel, the latter with
- * pixels on N, "tc" generic wgmma kernel, "simt" validation kernel, empty otherwise). `ms` is filled by calls made with option "time_ops" = 1
+ * pixels on N, "3x3_pair" persistent 3x3 kernel on (2,1,1) CTA-pair clusters (option conv3x3_2cta), "tc" generic
+ * wgmma kernel, "simt" validation kernel, empty otherwise; passes = 1 (hi x hi) or 3 (split
+ * product) for a category-0 conv, empty otherwise). `ms` is filled by calls made with option "time_ops" = 1
  * (eager run, one CUDA event pair per kernel on the launching stream), else -1.
  * *needed receives the buffer size required. */
 FILM_API int film_op_table(film_handle* h, char* buf, int64_t buf_size, int64_t* needed);
