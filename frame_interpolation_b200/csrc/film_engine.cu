@@ -1165,6 +1165,8 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
     P.release(feat[l]);  // the fusion-stage warp is the last reader of the feature level
     P.debug["aligned_side/" + std::to_string(l)] =
         DebugTensor{true, sd->hi, sd->lo, (int64_t)hh * ww, sd->C, 0, 10};
+    // every channel of the side tensor, the zero ones included (fusion_conv1 loads them against zero weights)
+    P.debug["out:fusion_side@L" + std::to_string(l)] = DebugTensor{true, sd->hi, sd->lo, (int64_t)hh * ww, sd->C, 0, sd->C};
     for (int k = 0; k < 2; ++k)
       P.debug["warped" + std::to_string(k) + "/" + std::to_string(l)] =
           DebugTensor{true, o->hi + (int64_t)k * hh * ww * C, o->lo + (int64_t)k * hh * ww * C, (int64_t)hh * ww, C, 0, C};
