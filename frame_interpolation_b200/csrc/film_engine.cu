@@ -594,8 +594,18 @@ struct Plan {
   std::map<std::string, DebugTensor> debug;
   float* xin = nullptr;   // [2][h][w][3] unpadded inputs
   float* xout = nullptr;  // [h][w][3]
+  float* time = nullptr;  // device scalar t of the fusion-stage warps: 0.5f (the reference's mid_time) unless a times call sets it
   cudaGraphExec_t graph = nullptr;
   double conv_flops = 0, mma_flops = 0, warp_bytes = 0, last_conv_bytes = 0;
+  // A times plan (film_interpolate_times) runs one head per frame pair and one tail per time.  ops[0, tail_begin) are the
+  // head (pad, pyramids, features, flows), ops[tail_begin, end) the tail (fusion warps, side tensors, decoder, RGB head),
+  // the only ops that read t.  The tail's inputs (img[], feat[0..4], v[]) are never recycled, so every replay of the tail
+  // reads what the head wrote.  With use_graph the head and the tail are captured as two graphs (graph, graph_tail).
+  bool times = false;
+  size_t tail_begin = 0;
+  int tok_head = -1;  // recorded after the last head op (use_lanes: joins the head's lanes before the first tail)
+  cudaGraphExec_t graph_tail = nullptr;
+  double head_conv_flops = 0, head_mma_flops = 0, head_warp_bytes = 0;  // the head's share of the three totals
 
   // Activation arena with liveness-based reuse.  The schedule is built in execution order and replayed on ONE
   // stream (or as the graph captured from it), so a buffer released at build position i may back any buffer
@@ -651,6 +661,7 @@ struct Plan {
 
   ~Plan() {
     if (graph) cudaGraphExecDestroy(graph);
+    if (graph_tail) cudaGraphExecDestroy(graph_tail);
     for (void* p : allocs) cudaFree(p);
   }
 };
@@ -881,10 +892,12 @@ static void padded_size(int h, int w, int align, int& H, int& W, int& off_y, int
   off_x = pw / 2;
 }
 
-static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align, const Options& opt, int num_sms) {
+static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align, const Options& opt, int num_sms,
+                                        bool times) {
   std::unique_ptr<Plan> pl(new Plan);
   Plan& P = *pl;
   P.opt = opt;
+  P.times = times;
   P.reuse = !opt.keep_debug && !opt.use_lanes && opt.arena_reuse;
   // the RGB head and the crop run in the epilogue of fusion_conv2@L0 instead of a kernel of their own
   const bool fuse_rgb = opt.conv_impl == 0 && opt.conv3x3_v2 && opt.fuse_rgb_head;
@@ -905,6 +918,12 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
 
   P.xin = P.alloc<float>((int64_t)2 * h * w * 3, true);
   P.xout = P.alloc<float>((int64_t)h * w * 3, true);
+  {  // four bytes outside the activation arena (arena_bytes is the arena's size)
+    const float half = 0.5f;
+    FILM_CUDA(cudaMalloc(&P.time, sizeof(float)));
+    P.allocs.push_back(P.time);
+    FILM_CUDA(cudaMemcpy(P.time, &half, sizeof(float), cudaMemcpyHostToDevice));
+  }
   Plan* pp = &P;
 
   // ---- image pyramids (util.py:23-45), both images batched: img[l] = [2][H_l][W_l][3]
@@ -1140,8 +1159,17 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
     P.debug["res_bwd/" + std::to_string(l)] = DebugTensor{false, res[l] + np * 2, nullptr, np, 2, 0, 2};
   }
 
+  if (times) {  // the cut: everything above ran once per frame pair, everything below runs once per time
+    P.tok_head = P.new_token();
+    P.signal_last(P.tok_head);
+    P.tail_begin = P.ops.size();
+    P.head_mma_flops = P.mma_flops;
+    P.head_warp_bytes = P.warp_bytes;
+  }
+
   // ---- fusion-stage warps (interpolator.py:153-183).  v[l] already equals the synthesised flow
   // pyramid of util.py:106-117 (same arithmetic, same order), so that pass is not repeated.
+  const float* tm = P.time;
   SplitBuf* wf[kFusionLevels];
   SplitBuf* side[kFusionLevels];
   for (int l = 0; l < kFusionLevels; ++l) {
@@ -1156,13 +1184,13 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
     const bool hi_only = P.hi_only(cons);
     const double wbytes = 2.0 * hh * ww * (double)C * (hi_only ? 4.0 : 8.0);
     P.add_op(1, "fusion_warp@L" + std::to_string(l), [=](cudaStream_t st) {
-      return launch_fusion_warp(vv, f->hi, f->lo, hh, ww, C, o->hi, o->lo, hi_only, st);
+      return launch_fusion_warp(vv, tm, f->hi, f->lo, hh, ww, C, o->hi, o->lo, hi_only, st);
     }, 0, wbytes);
     P.add_op(2, "fusion_side@L" + std::to_string(l), [=](cudaStream_t st) {
-      return launch_fusion_side(vv, im, hh, ww, sd->hi, sd->lo, sd->C, st);
+      return launch_fusion_side(vv, tm, im, hh, ww, sd->hi, sd->lo, sd->C, st);
     });
     P.warp_bytes += wbytes + 2.0 * hh * ww * 3.0 * 8.0;
-    P.release(feat[l]);  // the fusion-stage warp is the last reader of the feature level
+    if (!times) P.release(feat[l]);  // the fusion-stage warp is the last reader of the feature level (of one time)
     P.debug["aligned_side/" + std::to_string(l)] =
         DebugTensor{true, sd->hi, sd->lo, (int64_t)hh * ww, sd->C, 0, 10};
     // every channel of the side tensor, the zero ones included (fusion_conv1 loads them against zero weights)
@@ -1322,6 +1350,7 @@ static std::unique_ptr<Plan> build_plan(const Model& M, int h, int w, int align,
     }
     fu += (double)Hs[0] * Ws[0] * 64 * 3;
     P.conv_flops = 2.0 * (fe + fl + fu);
+    P.head_conv_flops = 2.0 * (fe + fl);
   }
 
   if (P.reuse)
@@ -1388,12 +1417,13 @@ static int fail(film_handle* h, const Error& e) noexcept {
   catch (const std::exception& e) { return fail(h, Error{FILM_ERR_CUDA, std::string("internal error: ") + e.what()}); } \
   catch (...) { return fail(h, Error{FILM_ERR_CUDA, "unknown internal error"}); }
 
-// Enqueues the whole schedule with `origin` as lane 0: fork the other lanes from it, express
-// cross-lane dependencies with events, join everything back into `origin`.  Works both eagerly and
-// under stream capture (the events become graph edges).
-static void enqueue_plan(film_handle* h, Plan* P, cudaStream_t origin) {
+// Enqueues ops [begin, end) of the schedule (all of it, or the head or the tail of a times plan) with `origin` as
+// lane 0: fork the other lanes from it, express cross-lane dependencies with events, join everything back into
+// `origin` through token `join` (recorded after the last op of the range).  Works both eagerly and under stream
+// capture (the events become graph edges).
+static void enqueue_plan(film_handle* h, Plan* P, cudaStream_t origin, size_t begin, size_t end, int join) {
   if (!h->opt.use_lanes) {
-    for (auto& op : P->ops) FILM_CUDA(op.fn(origin));
+    for (size_t i = begin; i < end; ++i) FILM_CUDA(P->ops[i].fn(origin));
     return;
   }
   if (!h->fork_event) FILM_CUDA(cudaEventCreateWithFlags(&h->fork_event, cudaEventDisableTiming));
@@ -1407,7 +1437,8 @@ static void enqueue_plan(film_handle* h, Plan* P, cudaStream_t origin) {
   auto lane_stream = [&](int lane) { return lane == 0 ? origin : h->lane_streams[lane]; };
   FILM_CUDA(cudaEventRecord(h->fork_event, origin));
   bool forked[Plan::kNumLanes] = {true};
-  for (auto& op : P->ops) {
+  for (size_t i = begin; i < end; ++i) {
+    const Plan::Op& op = P->ops[i];
     cudaStream_t st = lane_stream(op.lane);
     if (!forked[op.lane]) {
       FILM_CUDA(cudaStreamWaitEvent(st, h->fork_event, 0));
@@ -1417,7 +1448,7 @@ static void enqueue_plan(film_handle* h, Plan* P, cudaStream_t origin) {
     FILM_CUDA(op.fn(st));
     for (int t : op.signals) FILM_CUDA(cudaEventRecord(h->token_events[t], st));
   }
-  if (P->tok_end >= 0) FILM_CUDA(cudaStreamWaitEvent(origin, h->token_events[P->tok_end], 0));
+  if (join >= 0) FILM_CUDA(cudaStreamWaitEvent(origin, h->token_events[join], 0));
 }
 
 // Frees every cached plan (graphs + activation arenas) once the handle's stream has drained.
@@ -1430,7 +1461,8 @@ static void drop_plans(film_handle* h) {
   h->plans.clear();
 }
 
-static Plan* get_plan(film_handle* h, int hh, int ww, int align) {
+// `times`: the plan of film_interpolate_times (head and tail, see Plan::times), cached next to the ordinary plan
+static Plan* get_plan(film_handle* h, int hh, int ww, int align, bool times = false) {
   // Checked before the cache lookup: a plan built while any_size was 1 must not keep serving its size after the
   // option is set back to 0.  The plan itself does not depend on the option.
   if (!h->opt.any_size) {
@@ -1443,9 +1475,10 @@ static Plan* get_plan(film_handle* h, int hh, int ww, int align) {
   std::vector<int> key = {hh, ww, align > 0 ? align : 0};
   for (const OptionRow& r : kOptions)
     if (r.plan_key) key.push_back(h->opt.*r.field);
+  key.push_back(times ? 1 : 0);
   auto it = h->plans.find(key);
   if (it != h->plans.end()) return it->second.get();
-  auto build = [&] { return build_plan(*h->model, hh, ww, align, h->opt, h->num_sms); };
+  auto build = [&] { return build_plan(*h->model, hh, ww, align, h->opt, h->num_sms, times); };
   std::unique_ptr<Plan> p;
   try {
     p = build();
@@ -1456,11 +1489,11 @@ static Plan* get_plan(film_handle* h, int hh, int ww, int align) {
     drop_plans(h);
     p = build();
   }
-  if (h->opt.use_graph) {
+  auto capture = [&](size_t begin, size_t end, int join, cudaGraphExec_t* exec) {
     cudaGraph_t g = nullptr;
     FILM_CUDA(cudaStreamBeginCapture(h->stream, cudaStreamCaptureModeThreadLocal));
     try {
-      enqueue_plan(h, p.get(), h->stream);
+      enqueue_plan(h, p.get(), h->stream, begin, end, join);
     } catch (const Error& err) {
       cudaStreamEndCapture(h->stream, &g);
       if (g) cudaGraphDestroy(g);
@@ -1468,22 +1501,32 @@ static Plan* get_plan(film_handle* h, int hh, int ww, int align) {
       throw Error{FILM_ERR_CUDA, "kernel launch failed during capture: " + err.msg};
     }
     FILM_CUDA(cudaStreamEndCapture(h->stream, &g));
-    FILM_CUDA(cudaGraphInstantiate(&p->graph, g, 0));
+    const cudaError_t e = cudaGraphInstantiate(exec, g, 0);
     cudaGraphDestroy(g);
+    FILM_CUDA(e);
+  };
+  if (h->opt.use_graph) {
+    if (times) {
+      capture(0, p->tail_begin, p->tok_head, &p->graph);
+      capture(p->tail_begin, p->ops.size(), p->tok_end, &p->graph_tail);
+    } else {
+      capture(0, p->ops.size(), p->tok_end, &p->graph);
+    }
   }
   Plan* raw = p.get();
   h->plans[key] = std::move(p);
   return raw;
 }
 
-// runs the network of plan P on its xin -> xout (stream-ordered, not synchronised)
-static void run_plan(film_handle* h, Plan* P, cudaStream_t st) {
-  if (P->graph && !h->opt.time_ops) {  // a captured graph can be replayed on any stream
-    FILM_CUDA(cudaGraphLaunch(P->graph, st));
+// runs ops [begin, end) of plan P -- the whole network on its xin -> xout, or the head or the tail of a times plan --
+// as the captured graph `graph` (nullptr: eagerly).  Stream-ordered, not synchronised.
+static void run_ops(film_handle* h, Plan* P, cudaGraphExec_t graph, size_t begin, size_t end, int join, cudaStream_t st) {
+  if (graph && !h->opt.time_ops) {  // a captured graph can be replayed on any stream
+    FILM_CUDA(cudaGraphLaunch(graph, st));
   } else {
     if (h->opt.time_ops && st == h->stream) {
       // timed eager run: one event pair per op (bench.py's live per-kernel roofline numbers)
-      const size_t n = P->ops.size();
+      const size_t n = end - begin;
       while (h->op_events.size() < n + 1) {
         cudaEvent_t e;
         FILM_CUDA(cudaEventCreate(&e));
@@ -1491,18 +1534,21 @@ static void run_plan(film_handle* h, Plan* P, cudaStream_t st) {
       }
       FILM_CUDA(cudaEventRecord(h->op_events[0], st));
       for (size_t i = 0; i < n; ++i) {
-        FILM_CUDA(P->ops[i].fn(st));
+        FILM_CUDA(P->ops[begin + i].fn(st));
         FILM_CUDA(cudaEventRecord(h->op_events[i + 1], st));
       }
       FILM_CUDA(cudaStreamSynchronize(st));
-      P->op_ms.assign(n, 0.f);
-      for (size_t i = 0; i < n; ++i) FILM_CUDA(cudaEventElapsedTime(&P->op_ms[i], h->op_events[i], h->op_events[i + 1]));
+      if (P->op_ms.size() != P->ops.size()) P->op_ms.assign(P->ops.size(), 0.f);
+      for (size_t i = 0; i < n; ++i)
+        FILM_CUDA(cudaEventElapsedTime(&P->op_ms[begin + i], h->op_events[i], h->op_events[i + 1]));
     } else {
-      enqueue_plan(h, P, st);
+      enqueue_plan(h, P, st, begin, end, join);
     }
   }
   h->last_plan = P;
 }
+
+static void run_plan(film_handle* h, Plan* P, cudaStream_t st) { run_ops(h, P, P->graph, 0, P->ops.size(), P->tok_end, st); }
 
 extern "C" {
 
@@ -1796,6 +1842,109 @@ int film_interpolate_device(film_handle* h, const float* d_x0, const float* d_x1
       run_on_views(h, P, d_x0 + (int64_t)b * H * in_pitch, d_x1 + (int64_t)b * H * in_pitch, H, W, in_pitch,
                    d_out + (int64_t)b * H * out_pitch, out_pitch, st);
     fill_profile(h, P, -1.f, 0.f, 0.f);
+    h->dev_events_valid = true;
+    return FILM_OK;
+  }
+  FILM_CATCH_ALL(h)
+}
+
+// ---- film_interpolate_times: one head per frame pair, one tail per time (Plan::times)
+static void check_times(const float* times, int n_times) {
+  if (n_times < 1) throw Error{FILM_ERR_ARG, "n_times must be at least 1, got " + std::to_string(n_times)};
+  if (!times) throw Error{FILM_ERR_ARG, "null times pointer"};
+  for (int i = 0; i < n_times; ++i)
+    if (!(times[i] >= 0.f && times[i] <= 1.f)) {  // NaN fails both comparisons
+      char v[32];
+      snprintf(v, sizeof(v), "%.9g", (double)times[i]);
+      throw Error{FILM_ERR_ARG, "times[" + std::to_string(i) + "] = " + v + " is not a finite time in [0, 1]"};
+    }
+}
+
+extern "C++" {
+// The head of times plan P on its xin, then per time i: t_i into the plan's scalar, the tail, and `deliver(i, st)`, which
+// copies xout away before the next tail overwrites it.  ev[1] / ev[2] bracket the head, every tail and the deliveries.
+template <class Deliver>
+static void run_times(film_handle* h, Plan* P, const float* times, int n, cudaStream_t st, Deliver deliver) {
+  FILM_CUDA(cudaEventRecord(h->ev[1], st));
+  run_ops(h, P, P->graph, 0, P->tail_begin, P->tok_head, st);
+  for (int i = 0; i < n; ++i) {
+    FILM_CUDA(launch_set_time(P->time, times[i], st));
+    run_ops(h, P, P->graph_tail, P->tail_begin, P->ops.size(), P->tok_end, st);
+    deliver(i, st);
+  }
+  FILM_CUDA(cudaEventRecord(h->ev[2], st));
+}
+}  // extern "C++"
+
+// the profile of a whole times call: the head once, the tail n times
+static void fill_times_profile(film_handle* h, Plan* P, int n, float ms_net, float ms_h2d, float ms_d2h) {
+  fill_profile(h, P, ms_net, ms_h2d, ms_d2h);
+  film_profile_t& p = h->prof;
+  p.conv_flops = P->head_conv_flops + n * (P->conv_flops - P->head_conv_flops);
+  p.mma_flops = P->head_mma_flops + n * (P->mma_flops - P->head_mma_flops);
+  p.warp_bytes = P->head_warp_bytes + n * (P->warp_bytes - P->head_warp_bytes);
+  p.kernel_launches = (int64_t)P->tail_begin + (int64_t)n * (int64_t)(P->ops.size() - P->tail_begin);
+}
+
+int film_interpolate_times(film_handle* h, const float* x0, const float* x1, const float* times, int n_times, int H,
+                           int W, int align, float* out) {
+  if (!h) return FILM_ERR_ARG;
+  try {
+    check_frame_args(x0, x1, out, 1, H, W);
+    check_times(times, n_times);
+    FILM_CUDA(cudaSetDevice(h->device));
+    (void)cudaGetLastError();
+    Plan* P = get_plan(h, H, W, align, true);
+    const size_t frame = (size_t)H * W * 3 * sizeof(float);
+    ensure_staging(h, frame);
+    cudaStream_t ms = h->stream, cs = h->copy_stream;
+    FILM_CUDA(cudaStreamSynchronize(cs));
+    FILM_CUDA(cudaEventRecord(h->ev[0], ms));
+    FILM_CUDA(cudaMemcpyAsync(P->xin, x0, frame, cudaMemcpyHostToDevice, ms));
+    FILM_CUDA(cudaMemcpyAsync((char*)P->xin + frame, x1, frame, cudaMemcpyHostToDevice, ms));
+    // frame i leaves xout through staging slot i & 1; its download on the copy stream overlaps the tail of time i + 1
+    run_times(h, P, times, n_times, ms, [&](int i, cudaStream_t st) {
+      const int b = i & 1;
+      if (i >= 2) FILM_CUDA(cudaStreamWaitEvent(st, h->ev_out[b], 0));  // slot b drained by the download of frame i - 2
+      FILM_CUDA(cudaMemcpyAsync(h->stage_out[b], P->xout, frame, cudaMemcpyDeviceToDevice, st));
+      FILM_CUDA(cudaEventRecord(h->ev_done[b], st));
+      FILM_CUDA(cudaStreamWaitEvent(cs, h->ev_done[b], 0));
+      FILM_CUDA(cudaMemcpyAsync((char*)out + (size_t)i * frame, h->stage_out[b], frame, cudaMemcpyDeviceToHost, cs));
+      FILM_CUDA(cudaEventRecord(h->ev_out[b], cs));
+    });
+    FILM_CUDA(cudaEventRecord(h->ev[3], cs));
+    FILM_CUDA(cudaStreamSynchronize(cs));
+    FILM_CUDA(cudaStreamSynchronize(ms));
+    float ms_h2d, ms_net, ms_d2h;
+    FILM_CUDA(cudaEventElapsedTime(&ms_h2d, h->ev[0], h->ev[1]));
+    FILM_CUDA(cudaEventElapsedTime(&ms_net, h->ev[1], h->ev[2]));
+    FILM_CUDA(cudaEventElapsedTime(&ms_d2h, h->ev[2], h->ev[3]));
+    fill_times_profile(h, P, n_times, ms_net, ms_h2d, ms_d2h);
+    return FILM_OK;
+  }
+  FILM_CATCH_ALL(h)
+}
+
+int film_interpolate_times_device(film_handle* h, const float* d_x0, const float* d_x1, const float* times, int n_times,
+                                  int H, int W, int64_t in_pitch, int align, float* d_out, int64_t out_pitch,
+                                  void* cuda_stream) {
+  if (!h) return FILM_ERR_ARG;
+  try {
+    check_frame_args(d_x0, d_x1, d_out, 1, H, W);
+    check_times(times, n_times);
+    if (in_pitch < (int64_t)W * 3 || out_pitch < (int64_t)W * 3) throw Error{FILM_ERR_ARG, "pitch smaller than a row"};
+    FILM_CUDA(cudaSetDevice(h->device));
+    (void)cudaGetLastError();
+    Plan* P = get_plan(h, H, W, align, true);
+    cudaStream_t st = cuda_stream ? (cudaStream_t)cuda_stream : h->stream;
+    const size_t row = (size_t)W * 3 * sizeof(float);
+    FILM_CUDA(cudaMemcpy2DAsync(P->xin, row, d_x0, in_pitch * 4, row, H, cudaMemcpyDeviceToDevice, st));
+    FILM_CUDA(cudaMemcpy2DAsync(P->xin + (int64_t)H * W * 3, row, d_x1, in_pitch * 4, row, H, cudaMemcpyDeviceToDevice, st));
+    run_times(h, P, times, n_times, st, [&](int i, cudaStream_t s) {
+      FILM_CUDA(cudaMemcpy2DAsync(d_out + (int64_t)i * H * out_pitch, out_pitch * 4, P->xout, row, row, H,
+                                  cudaMemcpyDeviceToDevice, s));
+    });
+    fill_times_profile(h, P, n_times, -1.f, 0.f, 0.f);
     h->dev_events_valid = true;
     return FILM_OK;
   }

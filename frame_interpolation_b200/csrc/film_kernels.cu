@@ -661,10 +661,19 @@ cudaError_t launch_flow_warp(const float* v_prev, int Hc, int Wc, const sp_t* fe
 }
 
 // ------------------------------------------------------------------------------------------
-// interpolator.py:163-178  fusion-stage warps (flows scaled by 0.5)
+// interpolator.py:163-178  fusion-stage warps (interpolator.py:159-161: flows scaled by the time)
 // ------------------------------------------------------------------------------------------
+// multiply_pyramid (util.py:85-103) with mid_time = t: image 0 is read with fp32(t * bwd), image 1 with
+// fp32((1 - t) * fwd), 1 - t an fp32 subtraction.  The explicit intrinsics keep nvcc from contracting the product into
+// the coordinate add of warp_tap (an FMA would give another tap than the rounded flow the side tensor stores).  At
+// t = 0.5 both products are the exact halving.
+__device__ __forceinline__ float2 time_scaled_flow(float2 f, float t, int k) {
+  const float s = k == 0 ? t : __fsub_rn(1.f, t);
+  return make_float2(__fmul_rn(f.x, s), __fmul_rn(f.y, s));
+}
+
 template <bool kHiOnly>
-__global__ void __launch_bounds__(256) k_fusion_warp(const float* __restrict__ v,
+__global__ void __launch_bounds__(256) k_fusion_warp(const float* __restrict__ v, const float* __restrict__ time,
                                                      const sp_t* __restrict__ feat_hi,
                                                      const sp_t* __restrict__ feat_lo, int H, int W,
                                                      int C, sp_t* __restrict__ warped_hi,
@@ -676,9 +685,10 @@ __global__ void __launch_bounds__(256) k_fusion_warp(const float* __restrict__ v
   const int x = blockIdx.x * 8 + ((threadIdx.x >> 2) & 7), y = blockIdx.y * 8 + (threadIdx.x >> 5);
   if (x >= W || y >= H) return;
   const int64_t p = ((int64_t)k * H + y) * W + x;
-  // image k is warped by 0.5 * v[1 - k]
-  float2 f = __ldg(reinterpret_cast<const float2*>(v) + ((int64_t)(1 - k) * H + y) * W + x);
-  WarpTap t = warp_tap(y, x, f.x * 0.5f, f.y * 0.5f, H, W);
+  // image 0 is warped by t * v[1], image 1 by (1 - t) * v[0]
+  const float2 f = time_scaled_flow(__ldg(reinterpret_cast<const float2*>(v) + ((int64_t)(1 - k) * H + y) * W + x),
+                                    __ldg(time), k);
+  WarpTap t = warp_tap(y, x, f.x, f.y, H, W);
   const int64_t src_off = (int64_t)k * H * W * C;
   float o[16];
   if constexpr (kHiOnly) {
@@ -690,11 +700,18 @@ __global__ void __launch_bounds__(256) k_fusion_warp(const float* __restrict__ v
   }
 }
 
-cudaError_t launch_fusion_warp(const float* v, const sp_t* feat_hi, const sp_t* feat_lo, int H,
+cudaError_t launch_fusion_warp(const float* v, const float* time, const sp_t* feat_hi, const sp_t* feat_lo, int H,
                                int W, int C, sp_t* warped_hi, sp_t* warped_lo, bool hi_only, cudaStream_t st) {
   dim3 grid((W + 7) / 8, (H + 7) / 8, 2 * (C / 64));
-  if (hi_only) k_fusion_warp<true><<<grid, 256, 0, st>>>(v, feat_hi, feat_lo, H, W, C, warped_hi, warped_lo);
-  else k_fusion_warp<false><<<grid, 256, 0, st>>>(v, feat_hi, feat_lo, H, W, C, warped_hi, warped_lo);
+  if (hi_only) k_fusion_warp<true><<<grid, 256, 0, st>>>(v, time, feat_hi, feat_lo, H, W, C, warped_hi, warped_lo);
+  else k_fusion_warp<false><<<grid, 256, 0, st>>>(v, time, feat_hi, feat_lo, H, W, C, warped_hi, warped_lo);
+  return cudaGetLastError();
+}
+
+__global__ void k_set_time(float* __restrict__ time, float t) { *time = t; }
+
+cudaError_t launch_set_time(float* time, float t, cudaStream_t st) {
+  k_set_time<<<1, 1, 0, st>>>(time, t);
   return cudaGetLastError();
 }
 
@@ -741,7 +758,7 @@ cudaError_t launch_resize_nearest(const sp_t* src_hi, const sp_t* src_lo, int sr
   return cudaGetLastError();
 }
 
-__global__ void __launch_bounds__(256) k_fusion_side(const float* __restrict__ v,
+__global__ void __launch_bounds__(256) k_fusion_side(const float* __restrict__ v, const float* __restrict__ time,
                                                      const float* __restrict__ img, int H, int W,
                                                      sp_t* __restrict__ side_hi,
                                                      sp_t* __restrict__ side_lo, int side_C) {
@@ -749,14 +766,13 @@ __global__ void __launch_bounds__(256) k_fusion_side(const float* __restrict__ v
   int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= n) return;
   int x = (int)(p % W), y = (int)(p / W);
+  const float tm = __ldg(time);
   float o[16];
 #pragma unroll
   for (int j = 0; j < 16; ++j) o[j] = 0.f;
 #pragma unroll
   for (int k = 0; k < 2; ++k) {
-    float2 f = __ldg(reinterpret_cast<const float2*>(v) + ((int64_t)(1 - k) * H + y) * W + x);
-    f.x *= 0.5f;
-    f.y *= 0.5f;
+    const float2 f = time_scaled_flow(__ldg(reinterpret_cast<const float2*>(v) + ((int64_t)(1 - k) * H + y) * W + x), tm, k);
     WarpTap t = warp_tap(y, x, f.x, f.y, H, W);
     const float* ib = img + (int64_t)k * H * W * 3;
     const float* p00 = ib + ((int64_t)t.y0 * W + t.x0) * 3;
@@ -778,10 +794,10 @@ __global__ void __launch_bounds__(256) k_fusion_side(const float* __restrict__ v
   *reinterpret_cast<uint4*>(side_lo + oo + 8) = l;
 }
 
-cudaError_t launch_fusion_side(const float* v, const float* img, int H, int W, sp_t* side_hi,
+cudaError_t launch_fusion_side(const float* v, const float* time, const float* img, int H, int W, sp_t* side_hi,
                                sp_t* side_lo, int side_C, cudaStream_t st) {
   int64_t n = (int64_t)H * W;
-  k_fusion_side<<<cdiv(n, 256), 256, 0, st>>>(v, img, H, W, side_hi, side_lo, side_C);
+  k_fusion_side<<<cdiv(n, 256), 256, 0, st>>>(v, time, img, H, W, side_hi, side_lo, side_C);
   return cudaGetLastError();
 }
 

@@ -48,11 +48,13 @@ cudaError_t launch_flow_head(const sp_t* x_hi, const sp_t* x_lo, int Cx, int nf,
                              const float* w3, const float* b3, const float* w4, const float* b4,
                              const float* v_up, float* residual, float* v, cudaStream_t st);
 
-// interpolator.py:163-183: flows * 0.5, warp of [image, features] pyramids.
-// warped[k] = warp(feat[k], 0.5 * v[1-k])   (k = 0: image 0 by backward flow, k = 1: image 1
-// by forward flow; v[0] = forward flow, v[1] = backward flow).
-cudaError_t launch_fusion_warp(const float* v, const sp_t* feat_hi, const sp_t* feat_lo, int H,
+// interpolator.py:159-183: flows scaled by the time, warp of [image, features] pyramids.  `time` is a device scalar t
+// (0.5 in the reference graph): warped[0] = warp(feat[0], fp32(t * v[1])), warped[1] = warp(feat[1], fp32((1 - t) * v[0]))
+// (k = 0: image 0 by backward flow, k = 1: image 1 by forward flow; v[0] = forward flow, v[1] = backward flow).
+cudaError_t launch_fusion_warp(const float* v, const float* time, const sp_t* feat_hi, const sp_t* feat_lo, int H,
                                int W, int C, sp_t* warped_hi, sp_t* warped_lo, bool hi_only, cudaStream_t st);
+// one thread stores t into the device scalar `time`: stream-ordered, so a captured graph replayed after it reads t
+cudaError_t launch_set_time(float* time, float t, cudaStream_t st);
 // fusion.py:133 when the level is not exactly twice the coarser one: TF2 NEAREST resize of channels
 // [src_c_off, src_c_off + Cn) of a [B][Hi][Wi][src_C] split tensor into channels [dst_c_off, dst_c_off + Cn) of a
 // [B][Ho][Wo][dst_C] one, src = min(floor((dst + 0.5) * in / out), in - 1) per axis (exact integer arithmetic).
@@ -61,9 +63,9 @@ cudaError_t launch_fusion_warp(const float* v, const sp_t* feat_hi, const sp_t* 
 cudaError_t launch_resize_nearest(const sp_t* src_hi, const sp_t* src_lo, int src_C, int src_c_off, int B, int Hi, int Wi,
                                   sp_t* dst_hi, sp_t* dst_lo, int dst_C, int dst_c_off, int Ho, int Wo, int Cn, bool hi_only,
                                   cudaStream_t st);
-// side tensor [1][H][W][side_C] split: ch 0-2 warp(img0, .5*bwd), 3-5 warp(img1, .5*fwd),
-// 6-7 .5*bwd, 8-9 .5*fwd, 10-15 zero.
-cudaError_t launch_fusion_side(const float* v, const float* img, int H, int W, sp_t* side_hi,
+// side tensor [1][H][W][side_C] split: ch 0-2 warp(img0, t*bwd), 3-5 warp(img1, (1-t)*fwd),
+// 6-7 t*bwd, 8-9 (1-t)*fwd, 10-15 zero (t = *time, rounded like launch_fusion_warp).
+cudaError_t launch_fusion_side(const float* v, const float* time, const float* img, int H, int W, sp_t* side_hi,
                                sp_t* side_lo, int side_C, cudaStream_t st);
 
 // fusion.py:100-101,139 (1x1 conv 64 -> 3, linear) + crop (eval/interpolator.py:175).

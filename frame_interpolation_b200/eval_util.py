@@ -10,12 +10,17 @@ When the interpolator is the untiled engine, each pair's whole tree is evaluated
 device-resident call (`Interpolator.interpolate_recursively`): intermediate frames never leave
 HBM, which removes the per-mid-frame H2D + D2H + sync the reference pays
 (eval/interpolator.py:171,176). Any other callable `(x0, x1, dt) -> mid` takes the generic path.
+
+Frame-rate conversion (no reference counterpart): `retime_schedule` places every output frame of the target rate
+in a pair of input frames at an exact fractional time, and `retime_from_files` renders the sequence with one
+`interpolate_at` call per pair that needs frames.
 """
 from __future__ import annotations
 
 import os
 import shutil
-from typing import Callable, Iterable, Iterator, List, Sequence
+from fractions import Fraction
+from typing import Callable, Iterable, Iterator, List, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -99,6 +104,68 @@ def interpolate_recursively_from_files(frames: Sequence[str], times_to_interpola
         yield from _pair_sequence(prev, cur, times_to_interpolate, interpolator, progress)
         prev = cur
     yield prev
+
+
+Rate = Union[int, str, Fraction]
+
+
+def parse_rate(r: Rate) -> Fraction:
+    """A frame rate as an exact fraction: 30, "30", "29.97" or "24000/1001"."""
+    f = r if isinstance(r, Fraction) else Fraction(str(r))
+    assert f > 0, f"frame rates must be positive, got {r!r}"
+    return f
+
+
+def retime_schedule(n_frames: int, source_fps: Rate, target_fps: Rate) -> List[Tuple[int, Fraction]]:
+    """Output frame j of a clip of `n_frames` input frames converted from `source_fps` to `target_fps` sits at the
+    input position pos = j * source / target, for j = 0 .. floor((n_frames - 1) * target / source). Entry j is
+    (i, t): input pair (i, i + 1) at the exact time t = pos - i, i = floor(pos). t = 0 is input frame i itself
+    (the last input frame has i = n_frames - 1)."""
+    assert n_frames >= 1, "a clip needs at least one frame"
+    step = parse_rate(source_fps) / parse_rate(target_fps)
+    out = []
+    pos = Fraction(0)
+    while pos <= n_frames - 1:
+        i = pos.numerator // pos.denominator
+        out.append((i, pos - i))
+        pos += step
+    return out
+
+
+def retime_from_files(frames: Sequence[str], source_fps: Rate, target_fps: Rate, interpolator,
+                      progress=None) -> Iterator[np.ndarray]:
+    """Yields the clip `frames` (image files) retimed from `source_fps` to `target_fps` (see `retime_schedule`).
+    Every input pair that needs frames strictly between its ends gets ONE `interpolator.interpolate_at(frame_i,
+    frame_i1, times)` call for all of them; t = 0 yields the input frame without a network call. Only the current
+    pair is held in memory, and each file is decoded once."""
+    sched = retime_schedule(len(frames), source_fps, target_fps)
+    cur_i, cur, nxt = -1, None, None
+    k = 0
+    while k < len(sched):
+        i = sched[k][0]
+        if i != cur_i:  # advance to pair i: reuse the decoded right frame of the previous pair when it is frame i
+            cur = nxt if (nxt is not None and cur_i + 1 == i) else read_image(frames[i])
+            nxt = None
+            cur_i = i
+        ts = []
+        while k < len(sched) and sched[k][0] == i:
+            ts.append(sched[k][1])
+            k += 1
+        inner = [t for t in ts if t != 0]
+        mids = []
+        if inner:
+            nxt = read_image(frames[i + 1])
+            mids = interpolator.interpolate_at(cur, nxt, [float(t) for t in inner])
+            if progress:
+                progress(len(inner))
+        m = 0
+        for t in ts:
+            if t == 0:
+                yield cur
+            else:
+                # a copy, not a view: the result is one page-locked buffer of the engine's pool
+                yield np.array(mids[m])
+                m += 1
 
 
 def natural_sorted(names: Iterable[str]) -> List[str]:

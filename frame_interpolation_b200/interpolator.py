@@ -233,6 +233,43 @@ class Interpolator:
         self._check(st)
         return out
 
+    @staticmethod
+    def _times(times) -> np.ndarray:
+        return np.ascontiguousarray(np.asarray(times, dtype=np.float32).reshape(-1))
+
+    def interpolate_at(self, frame0: np.ndarray, frame1: np.ndarray, times) -> np.ndarray:
+        """Frames at arbitrary times between two (H, W, 3) frames: (len(times), H, W, 3) float32, frame i at times[i]
+        (each finite, 0 <= t <= 1). Frame i is the reference graph with its mid_time 0.5 replaced by times[i]
+        (film_interpolate_times): the features and both flow pyramids are computed once, the time-scaled warps and the
+        fusion decoder once per time. Bit-identical to `__call__` at t = 0.5; away from 0.5 the quality depends on the
+        weights, which the reference trained at t = 0.5 only. Untiled path."""
+        if self._align is not None:
+            assert self._align > 0, 'align must be a positive number.'
+        assert self._block_shape is None or np.prod(self._block_shape) <= 1, "interpolation at times is the untiled path"
+        f0 = np.ascontiguousarray(frame0, dtype=np.float32)
+        f1 = np.ascontiguousarray(frame1, dtype=np.float32)
+        assert f0.ndim == 3 and f0.shape == f1.shape and f0.shape[-1] == 3, "expected two (H, W, 3) frames"
+        t = self._times(times)
+        h, w, _ = f0.shape
+        out = self._pool.empty((max(t.shape[0], 1), h, w, 3))
+        st = self._lib.film_interpolate_times(self._handle, _fptr(f0), _fptr(f1), _fptr(t), t.shape[0], h, w,
+                                              int(self._align or 0), _fptr(out))
+        self._check(st)
+        return out
+
+    def interpolate_at_device(self, d_x0: int, d_x1: int, times, height: int, width: int, d_out: int,
+                              in_pitch: Optional[int] = None, out_pitch: Optional[int] = None, stream: int = 0) -> None:
+        """`interpolate_at` on device pointers (raw addresses, e.g. torch.Tensor.data_ptr()); asynchronous. Frame i is
+        written at d_out + i * height * out_pitch floats; `times` is read before the call returns."""
+        assert self._block_shape is None or np.prod(self._block_shape) <= 1, "interpolation at times is the untiled path"
+        t = self._times(times)
+        in_pitch = in_pitch or width * 3
+        out_pitch = out_pitch or width * 3
+        st = self._lib.film_interpolate_times_device(self._handle, C.c_void_p(d_x0), C.c_void_p(d_x1), _fptr(t),
+                                                     t.shape[0], height, width, in_pitch, int(self._align or 0),
+                                                     C.c_void_p(d_out), out_pitch, C.c_void_p(stream))
+        self._check(st)
+
     def interpolate_u8(self, x0: np.ndarray, x1: np.ndarray) -> np.ndarray:
         """8-bit in / 8-bit out: (B, H, W, 3) uint8 frames; the /255 of `read_image` (eval/util.py:38-41) and the
         quantisation of `write_image` (eval/util.py:51-52) run on the device, so PCIe carries a quarter of the bytes.

@@ -2,11 +2,17 @@
 
     python -m frame_interpolation_b200.interpolator_cli --pattern "photos" --model_path synthetic \
         --times_to_interpolate 3 [--align 64] [--block_height 2 --block_width 2 [--tile_overlap 32]] [--output_video --fps 30]
+    python -m frame_interpolation_b200.interpolator_cli --pattern "clips/*" --model_path film.filmw \
+        --source_fps 24 --target_fps 60 [--output_video]
 
 For every directory matching --pattern: the *.png/*.jpg/*.jpeg frames (natural order) are
 interpolated recursively and written to <dir>/interpolated_frames/frame_%03d.png
 (eval/interpolator_cli.py:127-177). No Beam runner: directories are processed in a loop, or, under
 torchrun, sharded over ranks (one GPU each). --output_video pipes frames to ffmpeg if present.
+
+With --source_fps S --target_fps T the frames are retimed instead (eval_util.retime_from_files): output frame j
+is the input clip at time j / T, interpolated at its exact fraction between two input frames, and the video is
+written at T fps. Away from the midpoint the quality depends on the weights (the reference trains at t = 0.5).
 """
 from __future__ import annotations
 
@@ -32,7 +38,8 @@ def build_parser() -> argparse.ArgumentParser:
                    help="FILMW1 weight file (tf_bundle.convert_saved_model output), or 'synthetic[:seed]' to opt in to "
                         "seeded random weights (plumbing tests only: the frames are meaningless).")
     p.add_argument("--times_to_interpolate", type=int, default=5,
-                   help="Number of recursive midpoint interpolations; output has 2^times+1 frames per input pair.")
+                   help="Number of recursive midpoint interpolations; output has 2^times+1 frames per input pair. "
+                        "Not used with --source_fps / --target_fps.")
     p.add_argument("--fps", type=int, default=30)
     p.add_argument("--align", type=int, default=64)
     p.add_argument("--block_height", type=int, default=1)
@@ -44,6 +51,11 @@ def build_parser() -> argparse.ArgumentParser:
                    help="With --block_height/--block_width: interpolate every tile on a window this many pixels larger on "
                         "each interior side and cross-fade neighbouring tiles over twice that width, instead of pasting "
                         "non-overlapping tiles like the reference (0, the default).")
+    p.add_argument("--source_fps", type=str, default=None,
+                   help="With --target_fps: retime the frames from this rate (e.g. 24, 29.97 or 24000/1001) instead of "
+                        "the recursive midpoint interpolation. Untiled only.")
+    p.add_argument("--target_fps", type=str, default=None,
+                   help="With --source_fps: the output frame rate, also the rate of --output_video.")
     p.add_argument("--output_video", action="store_true")
     p.add_argument("--device", type=int, default=None, help="CUDA device ordinal (default: LOCAL_RANK or 0)")
     return p
@@ -78,6 +90,19 @@ class _VideoWriter:
 def process_directory(directory: str, interpolator: Interpolator, times: int, fps: int, video: bool) -> int:
     """Frames are written (and piped to ffmpeg) as the generator yields them: nothing but the current input pair's
     sequence is ever held in memory (eval/interpolator_cli.py:164-177 materialises the whole list)."""
+    return _write_directory(directory, lambda names: eval_util.interpolate_recursively_from_files(names, times, interpolator),
+                            fps, video)
+
+
+def retime_directory(directory: str, interpolator: Interpolator, source_fps, target_fps, video: bool) -> int:
+    """The input frames retimed from `source_fps` to `target_fps` (eval_util.retime_from_files), written like
+    `process_directory`; the video runs at `target_fps`."""
+    target = eval_util.parse_rate(target_fps)
+    return _write_directory(directory, lambda names: eval_util.retime_from_files(names, source_fps, target, interpolator),
+                            target, video)
+
+
+def _write_directory(directory: str, sequence, fps, video: bool) -> int:
     names: List[str] = []
     for ext in _INPUT_EXT:
         names += eval_util.natural_sorted(glob.glob(os.path.join(directory, f"*.{ext}")))
@@ -92,7 +117,7 @@ def process_directory(directory: str, interpolator: Interpolator, times: int, fp
         os.makedirs(frames_dir)
     writer = None
     n = 0
-    for frame in eval_util.interpolate_recursively_from_files(names, times, interpolator):
+    for frame in sequence(names):
         eval_util.write_image(os.path.join(frames_dir, f"frame_{n:03d}.png"), frame)
         if video:
             if writer is None:
@@ -111,13 +136,21 @@ def main(argv=None) -> int:
     device = args.device if args.device is not None else int(os.environ.get("LOCAL_RANK", "0"))
     directories = sorted(d for d in glob.glob(args.pattern) if os.path.isdir(d))
     mine = directories[rank::world]            # directories are independent: shard them over ranks
+    retime = args.source_fps is not None or args.target_fps is not None
+    if retime and (args.source_fps is None or args.target_fps is None):
+        build_parser().error("--source_fps and --target_fps go together")
+    if retime and args.block_height * args.block_width > 1:
+        build_parser().error("--source_fps / --target_fps run untiled: drop --block_height / --block_width")
     interpolator = Interpolator(args.model_path, args.align, [args.block_height, args.block_width], device=device)
     if args.any_size:
         interpolator.set_option("any_size", 1)
     if args.tile_overlap:
         interpolator.set_option("tile_overlap", args.tile_overlap)
     for d in mine:
-        n = process_directory(d, interpolator, args.times_to_interpolate, args.fps, args.output_video)
+        if retime:
+            n = retime_directory(d, interpolator, args.source_fps, args.target_fps, args.output_video)
+        else:
+            n = process_directory(d, interpolator, args.times_to_interpolate, args.fps, args.output_video)
         print(f"[film_b200] {d}: wrote {n} frames to {d}/interpolated_frames", flush=True)
     return 0
 

@@ -134,6 +134,31 @@ FILM_API int film_stitch_tiles_device(film_handle* h, const float* d_tiles, int6
 FILM_API int film_interpolate_recursive(film_handle* h, const float* frame0, const float* frame1, int H, int W,
                                         int align, int times_to_interpolate, float* out);
 
+/* Frames at arbitrary times between two (H, W, 3) frames: frame i of `out` is the reference graph with mid_time
+ * (models/film_net/interpolator.py:159-161, multiply_pyramid) replaced by t_i = times[i]: image 0 is warped with
+ * fp32(t * backward_flow), image 1 with fp32((1 - t) * forward_flow) (1 - t an fp32 subtraction), and the side tensor,
+ * the warps and the fusion decoder follow.  No reference counterpart: the released weights were supervised at t = 0.5
+ * only, so the quality away from 0.5 depends on the weights.  At t = 0.5 frame i is bit-identical to film_interpolate on
+ * the same pair, handle options and align.
+ * One head (padding, pyramids, features, both flow pyramids) per call, then per time one tail (fusion warps, side
+ * tensors, decoder, RGB head); CUDA graphs: one for the head, one for the tail.  The times plan is cached next to the
+ * ordinary plan of the shape and keeps feature levels 0-4 of both images alive across the tails: 2.65 GB at 1088x1920
+ * (2 images x sum over levels 0-4 of H_l * W_l * C_l x 4 bytes, C_l = 64, 192, 448, 960, 960).  Its arena measured
+ * 0.94 GB larger than the ordinary plan's there (H100 80GB HBM3): the decoder finds most of its buffers in blocks the
+ * head has released.
+ * `times`: HOST array of n_times floats, read before the call returns.  Status 1 for n_times < 1 or a t that is not
+ * finite or not in [0, 1] (the message names its index); the frame-size rule (status 4 / option any_size) is the one of
+ * film_interpolate.  film_profile covers the whole call: conv_flops = head + n_times x tail, kernel_launches = head ops +
+ * n_times x tail ops (the one-thread kernel that stores each t is not counted).
+ * film_interpolate_times: host frames, `out` receives n_times frames; blocks until they are written.
+ * film_interpolate_times_device: device frames with row pitches like film_interpolate_device, frame i at
+ * d_out + i * H * out_pitch; asynchronous on `cuda_stream` (NULL = the handle's stream). */
+FILM_API int film_interpolate_times(film_handle* h, const float* x0, const float* x1, const float* times, int n_times,
+                                    int H, int W, int align, float* out);
+FILM_API int film_interpolate_times_device(film_handle* h, const float* d_x0, const float* d_x1, const float* times,
+                                           int n_times, int H, int W, int64_t in_pitch, int align, float* d_out,
+                                           int64_t out_pitch, void* cuda_stream);
+
 /* 8-bit front / back end (SURVEY 8f row 3): the frames cross PCIe as uint8 (4x fewer bytes) and the reference's
  * conversions run on the device, bit-identical to the host versions:
  *   in : float32 = uint8 / 255                         (eval/util.py:38-41, read_image)
