@@ -18,7 +18,7 @@ EXPORTS = [
     "film_debug_read", "film_op_table", "film_last_error", "film_version",
     "film_get_option", "film_stage_count", "film_stage_name",
     "film_interpolate_u8", "film_interpolate_recursive_u8", "film_stitch_tiles_device",
-    "film_interpolate_times", "film_interpolate_times_device",
+    "film_interpolate_times", "film_interpolate_times_device", "film_interpolate_times_tiled",
 ]
 
 
@@ -66,6 +66,9 @@ def load() -> C.CDLL:
     lib.film_interpolate_times_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, fp, C.c_int, C.c_int, C.c_int,
                                                   C.c_int64, C.c_int, C.c_void_p, C.c_int64, C.c_void_p]
     lib.film_interpolate_times_device.restype = C.c_int
+    lib.film_interpolate_times_tiled.argtypes = [C.c_void_p, fp, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                                 C.c_int, fp]
+    lib.film_interpolate_times_tiled.restype = C.c_int
     lib.film_interpolate_recursive.argtypes = [C.c_void_p, fp, fp, C.c_int, C.c_int, C.c_int, C.c_int, fp]
     lib.film_interpolate_recursive.restype = C.c_int
     up = C.POINTER(C.c_uint8)

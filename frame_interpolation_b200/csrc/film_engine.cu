@@ -2001,6 +2001,22 @@ int film_stitch_tiles_device(film_handle* h, const float* d_tiles, int64_t tile_
   FILM_CATCH_ALL(h)
 }
 
+// The handle's grow-only device scratch of the overlapped and the tiled times paths: at least `need` bytes.
+static float* ensure_overlap_stage(film_handle* h, size_t need, const char* what) {
+  if (h->overlap_bytes < need) {
+    if (h->overlap_stage) cudaFree(h->overlap_stage);
+    h->overlap_stage = nullptr;
+    h->overlap_bytes = 0;
+    if (cudaMalloc(&h->overlap_stage, need) != cudaSuccess) {
+      (void)cudaGetLastError();
+      h->overlap_stage = nullptr;
+      throw Error{FILM_ERR_CUDA, "out of device memory for the " + std::string(what) + ": " + std::to_string(need) + " bytes"};
+    }
+    h->overlap_bytes = need;
+  }
+  return h->overlap_stage;
+}
+
 // film_interpolate_tiled with tile_overlap > 0: both frames are uploaded once, every window runs as a pitched view of
 // the resident frames into a [tiles][q_h][q_w][3] buffer, one kernel stitches that buffer into a device frame, one
 // download.  The scratch memory belongs to the handle.
@@ -2011,15 +2027,8 @@ static void interpolate_tiled_overlapped(film_handle* h, const float* x0, const 
   (void)cudaGetLastError();
   Plan* P = get_plan(h, qh, qw, align);
   const size_t frame = (size_t)H * W * 3, window = (size_t)qh * qw * 3;  // floats
-  const size_t need = (3 * frame + nt * window) * sizeof(float);
-  if (h->overlap_bytes < need) {
-    if (h->overlap_stage) cudaFree(h->overlap_stage);
-    h->overlap_stage = nullptr;
-    h->overlap_bytes = 0;
-    FILM_CUDA(cudaMalloc(&h->overlap_stage, need));
-    h->overlap_bytes = need;
-  }
-  float *d0 = h->overlap_stage, *d1 = d0 + frame, *d_out = d1 + frame, *d_tiles = d_out + frame;
+  float* d0 = ensure_overlap_stage(h, (3 * frame + nt * window) * sizeof(float), "overlapped tiles (3 frames, tiles windows)");
+  float *d1 = d0 + frame, *d_out = d1 + frame, *d_tiles = d_out + frame;
   cudaStream_t st = h->stream;
   FILM_CUDA(cudaMemcpyAsync(d0, x0, frame * sizeof(float), cudaMemcpyHostToDevice, st));
   FILM_CUDA(cudaMemcpyAsync(d1, x1, frame * sizeof(float), cudaMemcpyHostToDevice, st));
@@ -2090,6 +2099,59 @@ int film_interpolate_tiled(film_handle* h, const float* x0, const float* x1, con
         ms_d2h += t;
       }
     fill_profile(h, P, ms_net, ms_h2d, ms_d2h);
+    return FILM_OK;
+  }
+  FILM_CATCH_ALL(h)
+}
+
+// film_interpolate_times on the windows of film_interpolate_tiled: both frames are uploaded once, every window (row-major)
+// runs one head and n tails of the one times plan of the window shape, each tail's result lands in a time-major
+// [n][tiles][q_h][q_w][3] buffer, and one stitch per time blends that time's windows into a device frame.  At overlap 0
+// the windows are the reference's tiles and the stitch is a paste.  The scratch memory is the handle's overlap_stage.
+int film_interpolate_times_tiled(film_handle* h, const float* x0, const float* x1, const float* times, int n_times,
+                                 int H, int W, int align, int block_h, int block_w, float* out) {
+  if (!h) return FILM_ERR_ARG;
+  try {
+    check_frame_args(x0, x1, out, 1, H, W);
+    check_times(times, n_times);
+    const StitchGeom g = stitch_geometry(H, W, block_h, block_w, h->opt.tile_overlap, nullptr);
+    const int qh = g.ay.q, qw = g.ax.q, nt = block_h * block_w;
+    FILM_CUDA(cudaSetDevice(h->device));
+    (void)cudaGetLastError();
+    Plan* P = get_plan(h, qh, qw, align, true);
+    const size_t frame = (size_t)H * W * 3, window = (size_t)qh * qw * 3;  // floats
+    float* d0 = ensure_overlap_stage(h, ((2 + (size_t)n_times) * frame + (size_t)n_times * nt * window) * sizeof(float),
+                                     "tiled times ((2 + n_times) frames, n_times x tiles windows)");
+    float *d1 = d0 + frame, *d_frames = d1 + frame, *d_tiles = d_frames + n_times * frame;
+    cudaStream_t st = h->stream;
+    const size_t row = (size_t)qw * 3 * sizeof(float);
+    FILM_CUDA(cudaMemcpyAsync(d0, x0, frame * sizeof(float), cudaMemcpyHostToDevice, st));
+    FILM_CUDA(cudaMemcpyAsync(d1, x1, frame * sizeof(float), cudaMemcpyHostToDevice, st));
+    FILM_CUDA(cudaEventRecord(h->ev[0], st));
+    for (int t = 0; t < nt; ++t) {  // row-major tile order, like film_interpolate_tiled
+      const size_t off = ((size_t)stitch_origin(g.ay, t / block_w) * W + stitch_origin(g.ax, t % block_w)) * 3;
+      FILM_CUDA(cudaMemcpy2DAsync(P->xin, row, d0 + off, (size_t)W * 3 * sizeof(float), row, qh, cudaMemcpyDeviceToDevice, st));
+      FILM_CUDA(cudaMemcpy2DAsync(P->xin + window, row, d1 + off, (size_t)W * 3 * sizeof(float), row, qh,
+                                  cudaMemcpyDeviceToDevice, st));
+      run_times(h, P, times, n_times, st, [&](int i, cudaStream_t s) {
+        FILM_CUDA(cudaMemcpyAsync(d_tiles + ((size_t)i * nt + t) * window, P->xout, window * sizeof(float),
+                                  cudaMemcpyDeviceToDevice, s));
+      });
+    }
+    for (int i = 0; i < n_times; ++i)  // time i's windows sit at d_tiles + i * nt * window, one window apart
+      FILM_CUDA(launch_stitch_feather(d_tiles + (size_t)i * nt * window, (int64_t)window, g, d_frames + i * frame,
+                                      (int64_t)W * 3, st));
+    FILM_CUDA(cudaEventRecord(h->ev[3], st));
+    FILM_CUDA(cudaMemcpyAsync(out, d_frames, n_times * frame * sizeof(float), cudaMemcpyDeviceToHost, st));
+    FILM_CUDA(cudaStreamSynchronize(st));
+    float ms_net = 0;
+    FILM_CUDA(cudaEventElapsedTime(&ms_net, h->ev[0], h->ev[3]));
+    fill_times_profile(h, P, n_times, ms_net, 0.f, 0.f);
+    film_profile_t& p = h->prof;  // every window ran one head and n tails
+    p.conv_flops *= nt;
+    p.mma_flops *= nt;
+    p.warp_bytes *= nt;
+    p.kernel_launches *= nt;
     return FILM_OK;
   }
   FILM_CATCH_ALL(h)

@@ -133,11 +133,13 @@ def retime_schedule(n_frames: int, source_fps: Rate, target_fps: Rate) -> List[T
 
 
 def retime_from_files(frames: Sequence[str], source_fps: Rate, target_fps: Rate, interpolator,
-                      progress=None) -> Iterator[np.ndarray]:
+                      progress=None, at: Callable | None = None) -> Iterator[np.ndarray]:
     """Yields the clip `frames` (image files) retimed from `source_fps` to `target_fps` (see `retime_schedule`).
-    Every input pair that needs frames strictly between its ends gets ONE `interpolator.interpolate_at(frame_i,
-    frame_i1, times)` call for all of them; t = 0 yields the input frame without a network call. Only the current
-    pair is held in memory, and each file is decoded once."""
+    Every input pair that needs frames strictly between its ends gets ONE `at(frame_i, frame_i1, times)` call for all
+    of them (default `interpolator.interpolate_at`; `interpolator.interpolate_at_tiled` for tiles); t = 0 yields the
+    input frame without a network call. Only the current pair is held in memory, and each file is decoded once."""
+    if at is None:
+        at = interpolator.interpolate_at
     sched = retime_schedule(len(frames), source_fps, target_fps)
     cur_i, cur, nxt = -1, None, None
     k = 0
@@ -155,7 +157,7 @@ def retime_from_files(frames: Sequence[str], source_fps: Rate, target_fps: Rate,
         mids = []
         if inner:
             nxt = read_image(frames[i + 1])
-            mids = interpolator.interpolate_at(cur, nxt, [float(t) for t in inner])
+            mids = at(cur, nxt, [float(t) for t in inner])
             if progress:
                 progress(len(inner))
         m = 0

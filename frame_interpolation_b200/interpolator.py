@@ -242,20 +242,40 @@ class Interpolator:
         (each finite, 0 <= t <= 1). Frame i is the reference graph with its mid_time 0.5 replaced by times[i]
         (film_interpolate_times): the features and both flow pyramids are computed once, the time-scaled warps and the
         fusion decoder once per time. Bit-identical to `__call__` at t = 0.5; away from 0.5 the quality depends on the
-        weights, which the reference trained at t = 0.5 only. Untiled path."""
+        weights, which the reference trained at t = 0.5 only. Untiled path: a tiled engine uses `interpolate_at_tiled`."""
         if self._align is not None:
             assert self._align > 0, 'align must be a positive number.'
         assert self._block_shape is None or np.prod(self._block_shape) <= 1, "interpolation at times is the untiled path"
-        f0 = np.ascontiguousarray(frame0, dtype=np.float32)
-        f1 = np.ascontiguousarray(frame1, dtype=np.float32)
-        assert f0.ndim == 3 and f0.shape == f1.shape and f0.shape[-1] == 3, "expected two (H, W, 3) frames"
-        t = self._times(times)
+        f0, f1, t = self._times_args(frame0, frame1, times)
         h, w, _ = f0.shape
         out = self._pool.empty((max(t.shape[0], 1), h, w, 3))
         st = self._lib.film_interpolate_times(self._handle, _fptr(f0), _fptr(f1), _fptr(t), t.shape[0], h, w,
                                               int(self._align or 0), _fptr(out))
         self._check(st)
         return out
+
+    def interpolate_at_tiled(self, frame0: np.ndarray, frame1: np.ndarray, times) -> np.ndarray:
+        """`interpolate_at` on the engine's tiles (block_shape, None meaning [1, 1], and option tile_overlap):
+        (len(times), H, W, 3) float32, frame i what `__call__` computes on the tiles with every window's mid_time
+        replaced by times[i] (film_interpolate_times_tiled). One head and n tails per window, one stitch per time.
+        Bit-identical to `__call__` at t = 0.5; at tile_overlap 0, tile k of frame i is `interpolate_at` on tile k's
+        crop."""
+        if self._align is not None:
+            assert self._align > 0, 'align must be a positive number.'
+        f0, f1, t = self._times_args(frame0, frame1, times)
+        h, w, _ = f0.shape
+        bh, bw = (int(self._block_shape[0]), int(self._block_shape[1])) if self._block_shape is not None else (1, 1)
+        out = self._pool.empty((max(t.shape[0], 1), h, w, 3))
+        st = self._lib.film_interpolate_times_tiled(self._handle, _fptr(f0), _fptr(f1), _fptr(t), t.shape[0], h, w,
+                                                    int(self._align or 0), bh, bw, _fptr(out))
+        self._check(st)
+        return out
+
+    def _times_args(self, frame0, frame1, times):
+        f0 = np.ascontiguousarray(frame0, dtype=np.float32)
+        f1 = np.ascontiguousarray(frame1, dtype=np.float32)
+        assert f0.ndim == 3 and f0.shape == f1.shape and f0.shape[-1] == 3, "expected two (H, W, 3) frames"
+        return f0, f1, self._times(times)
 
     def interpolate_at_device(self, d_x0: int, d_x1: int, times, height: int, width: int, d_out: int,
                               in_pitch: Optional[int] = None, out_pitch: Optional[int] = None, stream: int = 0) -> None:

@@ -3,7 +3,7 @@
     python -m frame_interpolation_b200.interpolator_cli --pattern "photos" --model_path synthetic \
         --times_to_interpolate 3 [--align 64] [--block_height 2 --block_width 2 [--tile_overlap 32]] [--output_video --fps 30]
     python -m frame_interpolation_b200.interpolator_cli --pattern "clips/*" --model_path film.filmw \
-        --source_fps 24 --target_fps 60 [--output_video]
+        --source_fps 24 --target_fps 60 [--block_height 2 --block_width 2 --tile_overlap 32] [--output_video]
 
 For every directory matching --pattern: the *.png/*.jpg/*.jpeg frames (natural order) are
 interpolated recursively and written to <dir>/interpolated_frames/frame_%03d.png
@@ -13,6 +13,8 @@ torchrun, sharded over ranks (one GPU each). --output_video pipes frames to ffmp
 With --source_fps S --target_fps T the frames are retimed instead (eval_util.retime_from_files): output frame j
 is the input clip at time j / T, interpolated at its exact fraction between two input frames, and the video is
 written at T fps. Away from the midpoint the quality depends on the weights (the reference trains at t = 0.5).
+Tiled retiming (Interpolator.interpolate_at_tiled) needs --tile_overlap > 0: pasted tiles disagree along every seam, and
+in a retimed clip that disagreement changes with t from frame to frame, so it shows as a flickering line.
 """
 from __future__ import annotations
 
@@ -53,7 +55,8 @@ def build_parser() -> argparse.ArgumentParser:
                         "non-overlapping tiles like the reference (0, the default).")
     p.add_argument("--source_fps", type=str, default=None,
                    help="With --target_fps: retime the frames from this rate (e.g. 24, 29.97 or 24000/1001) instead of "
-                        "the recursive midpoint interpolation. Untiled only.")
+                        "the recursive midpoint interpolation. With --block_height/--block_width it needs --tile_overlap "
+                        "> 0.")
     p.add_argument("--target_fps", type=str, default=None,
                    help="With --source_fps: the output frame rate, also the rate of --output_video.")
     p.add_argument("--output_video", action="store_true")
@@ -94,11 +97,13 @@ def process_directory(directory: str, interpolator: Interpolator, times: int, fp
                             fps, video)
 
 
-def retime_directory(directory: str, interpolator: Interpolator, source_fps, target_fps, video: bool) -> int:
-    """The input frames retimed from `source_fps` to `target_fps` (eval_util.retime_from_files), written like
-    `process_directory`; the video runs at `target_fps`."""
+def retime_directory(directory: str, interpolator: Interpolator, source_fps, target_fps, video: bool, at=None) -> int:
+    """The input frames retimed from `source_fps` to `target_fps` (eval_util.retime_from_files, each pair's frames
+    from `at`, default `interpolator.interpolate_at`), written like `process_directory`; the video runs at
+    `target_fps`."""
     target = eval_util.parse_rate(target_fps)
-    return _write_directory(directory, lambda names: eval_util.retime_from_files(names, source_fps, target, interpolator),
+    return _write_directory(directory,
+                            lambda names: eval_util.retime_from_files(names, source_fps, target, interpolator, at=at),
                             target, video)
 
 
@@ -139,8 +144,12 @@ def main(argv=None) -> int:
     retime = args.source_fps is not None or args.target_fps is not None
     if retime and (args.source_fps is None or args.target_fps is None):
         build_parser().error("--source_fps and --target_fps go together")
-    if retime and args.block_height * args.block_width > 1:
-        build_parser().error("--source_fps / --target_fps run untiled: drop --block_height / --block_width")
+    tiled = args.block_height * args.block_width > 1
+    if retime and tiled and args.tile_overlap <= 0:
+        # pasted tiles disagree along every seam, and in a retimed clip that disagreement changes with t from frame to
+        # frame: a flickering line
+        build_parser().error("tiled retiming (--source_fps / --target_fps with --block_height / --block_width) needs "
+                             "--tile_overlap > 0")
     interpolator = Interpolator(args.model_path, args.align, [args.block_height, args.block_width], device=device)
     if args.any_size:
         interpolator.set_option("any_size", 1)
@@ -148,7 +157,8 @@ def main(argv=None) -> int:
         interpolator.set_option("tile_overlap", args.tile_overlap)
     for d in mine:
         if retime:
-            n = retime_directory(d, interpolator, args.source_fps, args.target_fps, args.output_video)
+            n = retime_directory(d, interpolator, args.source_fps, args.target_fps, args.output_video,
+                                 at=interpolator.interpolate_at_tiled if tiled else None)
         else:
             n = process_directory(d, interpolator, args.times_to_interpolate, args.fps, args.output_video)
         print(f"[film_b200] {d}: wrote {n} frames to {d}/interpolated_frames", flush=True)

@@ -11,6 +11,7 @@ The path shards into independent units:
   the stitched frame (NCCL over NVLink on GPUs; gloo on CPU for the host-logic tests).
   With `overlap` > 0 every tile runs on its window of `spec.tile_windows` and the gathered
   results are cross-faded instead of pasted (engine option tile_overlap).
+  `interpolate_at_tiled_device` is the same for the frames of one pair at several times.
 * recursion    -- `interpolate_recursively`: eval/util.py:62-91's binary dependency tree
   scheduled level-synchronously: the 2^(k-1) calls of level k are sharded, new mid-frames
   are all-gathered so every rank holds the parents of level k+1; the output order is the
@@ -184,25 +185,54 @@ def device_engine(interp):
         for t in (x0, x1, out):
             t.record_stream(es)
 
+    def at(x0, x1, times, out):
+        """Frames of (x0, x1) at `times` (`Interpolator.interpolate_at_device`) into the dense (n, H, W, 3) tensor `out`,
+        frame i at out[i]; same stream semantics as the network call. The Interpolator must be untiled."""
+        h, w, _ = x0.shape
+        n = len(times)
+        for t in (x0, x1):
+            assert t.dtype == torch.float32 and t.is_cuda and t.shape == (h, w, 3)
+            assert t.stride(2) == 1 and t.stride(1) == 3, "inner dims must be dense (row-pitched view)"
+        assert x0.stride(0) == x1.stride(0), "x0 and x1 must share the row pitch"
+        assert out.dtype == torch.float32 and out.is_cuda and out.shape == (n, h, w, 3) and out.is_contiguous()
+        dev = x0.device
+        if dev not in side:
+            side[dev] = torch.cuda.Stream(device=dev)
+        es, cur = side[dev], torch.cuda.current_stream(dev)
+        es.wait_stream(cur)
+        interp.interpolate_at_device(x0.data_ptr(), x1.data_ptr(), times, h, w, out.data_ptr(), in_pitch=x0.stride(0),
+                                     out_pitch=w * 3, stream=es.cuda_stream)
+        cur.wait_stream(es)
+        for t in (x0, x1, out):
+            t.record_stream(es)
+
     def stitch(tiles, slot_of_tile, block_shape, overlap, out):
         """Feathered stitch (film_stitch_tiles_device) of the window results in `tiles` (slots, q_h, q_w, 3), tile t in
-        slot slot_of_tile[t], into the (H, W, 3) view `out`; same stream semantics as the network call."""
+        slot slot_of_tile[t], into the (H, W, 3) view `out`; same stream semantics as the network call. The inner three
+        dims of `tiles` must be dense; the slots may be further apart (tile_stride = tiles.stride(0)), so a per-time
+        slice of a gather buffer is read in place."""
         h, w, _ = out.shape
         qh, qw = tiles.shape[-3], tiles.shape[-2]
-        assert tiles.dtype == out.dtype == torch.float32 and tiles.is_cuda and tiles.is_contiguous()
+        if tiles.dim() != 4:
+            assert tiles.is_contiguous(), "tiles must be (slots, q_h, q_w, 3) or contiguous"
+            tiles = tiles.view(-1, qh, qw, 3)
+        assert tiles.dtype == out.dtype == torch.float32 and tiles.is_cuda
+        assert tiles.stride(3) == 1 and tiles.stride(2) == 3 and tiles.stride(1) == qw * 3, "inner dims must be dense"
         assert (qh, qw) == spec.tile_windows(h, w, block_shape, overlap)[1], "tiles do not have the window shape"
-        assert max(slot_of_tile) < tiles.numel() // (qh * qw * 3), "slot outside the tile buffer"
+        assert max(slot_of_tile) < tiles.shape[0], "slot outside the tile buffer"
         assert out.stride(2) == 1 and out.stride(1) == 3, "inner dims must be dense (row-pitched view)"
         dev = out.device
         if dev not in side:
             side[dev] = torch.cuda.Stream(device=dev)
         es, cur = side[dev], torch.cuda.current_stream(dev)
         es.wait_stream(cur)
-        interp.stitch_tiles_device(tiles.data_ptr(), qh * qw * 3, h, w, block_shape, overlap, out.data_ptr(),
-                                   slot_of_tile=slot_of_tile, out_pitch=out.stride(0), stream=es.cuda_stream)
+        interp.stitch_tiles_device(tiles.data_ptr(), max(tiles.stride(0), qh * qw * 3), h, w, block_shape, overlap,
+                                   out.data_ptr(), slot_of_tile=slot_of_tile, out_pitch=out.stride(0),
+                                   stream=es.cuda_stream)
         cur.wait_stream(es)
         for t in (tiles, out):
             t.record_stream(es)
+    run.at = at
     run.stitch = stitch
     return run
 
@@ -273,6 +303,36 @@ def interpolate_tiled_device(engine_dev, x0, x1, block_shape, group=None, out=No
     # slot [r, j] holds tile j * world + r -> tile-major order, then patches_to_image as one strided copy
     tiles = gather_buf.transpose(0, 1).reshape(world * m, ph, pw, 3)[:nt]
     out.view(bh, ph, bw, pw, 3).copy_(tiles.view(bh, bw, ph, pw, 3).permute(0, 2, 1, 3, 4))
+    return out
+
+
+def interpolate_at_tiled_device(engine_dev, x0, x1, times, block_shape, group=None, out=None, gather_buf=None, overlap=0):
+    """The times form of `interpolate_tiled_device`: frames of one pair at every t in `times`, tiled, device-resident.
+
+    x0, x1: (1, H, W, 3) or (H, W, 3) tensors resident on every rank's device. Tiles go round-robin over ranks; rank r
+    runs `engine_dev.at` (one head and n tails, `device_engine` over an untiled Interpolator) on the windows of
+    `spec.tile_windows` of its tiles, straight into slot [r, j] of the (world, m, n, q_h, q_w, 3) gather buffer; ONE
+    all-gather; then one `engine_dev.stitch` per time reads that time's slots in place through the slot table (a paste
+    at overlap 0). Returns `out`, (n, H, W, 3), allocated if None."""
+    import torch
+    world, rank = _world_rank(group)
+    bh, bw = int(block_shape[0]), int(block_shape[1])
+    nt, n = bh * bw, len(times)
+    h, w = x0.shape[-3], x0.shape[-2]
+    qh, qw = spec.tile_windows(h, w, [bh, bw], overlap)[1]
+    m = (nt + world - 1) // world
+    if gather_buf is None:
+        gather_buf = torch.empty((world, m, n, qh, qw, 3), dtype=torch.float32, device=x0.device)
+    for j, t in enumerate(round_robin(nt, world, rank)):
+        engine_dev.at(window_view(x0, block_shape, t, overlap), window_view(x1, block_shape, t, overlap), times,
+                      gather_buf[rank, j])
+    _all_gather_slots(gather_buf, group)
+    if out is None:
+        out = torch.empty((n, h, w, 3), dtype=torch.float32, device=x0.device)
+    slots = [(t % world) * m + t // world for t in range(nt)]   # slot [r, j] holds tile j * world + r
+    per_time = gather_buf.view(world * m, n, qh, qw, 3)
+    for i in range(n):
+        engine_dev.stitch(per_time[:, i], slots, [bh, bw], overlap, out[i])
     return out
 
 

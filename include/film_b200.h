@@ -159,6 +159,27 @@ FILM_API int film_interpolate_times_device(film_handle* h, const float* d_x0, co
                                            int n_times, int H, int W, int64_t in_pitch, int align, float* d_out,
                                            int64_t out_pitch, void* cuda_stream);
 
+/* film_interpolate_times on the tiles of film_interpolate_tiled: frame i of `out` is what film_interpolate_tiled computes
+ * with the handle's "tile_overlap" v, with every window's mid_time replaced by t_i = times[i].  The windows are those of
+ * film_stitch_tiles_device (v = 0: the reference's non-overlapping tiles, each padded on its own to `align`); every
+ * window runs what film_interpolate_times runs on its crop, one head and then one tail per time, and per time the window
+ * results are stitched by film_stitch_tiles_device (a paste at v = 0).  Consequences: at t = 0.5 frame i is bit-identical
+ * to film_interpolate_tiled on the same pair, options, align and overlap; at v = 0 tile k of frame i is bit-identical to
+ * film_interpolate_times on tile k's crop; block 1 x 1 is film_interpolate_times.
+ * Host frames in; `out` receives n_times frames of (H, W, 3); blocks until they are written.  Both frames are uploaded
+ * once, and one times plan of the window shape serves every window (row-major order).  Times are checked as in
+ * film_interpolate_times, the geometry as in film_interpolate_tiled (divisibility, 2v <= tile size on every blocked
+ * axis, at most 64 tiles: status 1); the frame-size rule (status 4 / option any_size) applies to the window shape.
+ * Device scratch, kept by the handle and grown on demand: (2 + n_times) frames plus n_times x tiles windows of float32,
+ * i.e. 4 x ((2 + n) x H x W x 3 + n x tiles x q_h x q_w x 3) bytes (8K in 4x4 tiles at v = 0 and n = 7: 9 x 398 MB + 112 x
+ * 24.9 MB = 6.4 GB, next to the times plan of the window); a failed allocation is status 2 and names the bytes.
+ * film_profile covers the whole call: conv_flops = tiles x (head + n_times x tail), kernel_launches = tiles x (head ops +
+ * n_times x tail ops) (the kernels that store t and the stitches are not counted), padded_h / padded_w = the padded
+ * window, last_call_ms = every window's network plus the stitches (uploads and download excluded).  With option
+ * keep_debug, film_debug_read returns the last window's last time. */
+FILM_API int film_interpolate_times_tiled(film_handle* h, const float* x0, const float* x1, const float* times,
+                                          int n_times, int H, int W, int align, int block_h, int block_w, float* out);
+
 /* 8-bit front / back end (SURVEY 8f row 3): the frames cross PCIe as uint8 (4x fewer bytes) and the reference's
  * conversions run on the device, bit-identical to the host versions:
  *   in : float32 = uint8 / 255                         (eval/util.py:38-41, read_image)
