@@ -108,8 +108,9 @@ struct alignas(64) ConvProblem {
   int straight;           // persistent kernel, resident weights: 1 = a whole activation stage is one wgmma group issued as
                           // straight-line code (default), 0 = one group per tap
   int out_lo_skip;        // 1: every consumer of the destination reads the hi plane only -> the lo plane is not written
-  int pxn;                // persistent kernel, Cout = 64, 64-channel chunks, store / pool epilogue: 1 = pixels on the wgmma N
-                          // dimension (D^T = W_tap x A^T, m64n128k16, 32x8 tiles of 128 pixels per consumer warpgroup)
+  int pxn;                // persistent kernel, BN = 64 or 128, 64-channel chunks, store / pool epilogue: 1 = pixels on the
+                          // wgmma N dimension (D^T = W_tap x A^T, one m64n128k16 per 64-cout half of the N tile, 32x8 tiles
+                          // of 128 pixels per consumer warpgroup)
 };
 
 // launchers (film_conv_tc.cu / film_kernels.cu)

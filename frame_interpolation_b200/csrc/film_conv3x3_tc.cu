@@ -14,14 +14,17 @@
 //    the consumers drain the accumulators of the current one.
 //  * Two-accumulator product (BN <= 128): A_hi x W_hi and A_lo x W_hi accumulate into columns [0, BN) and A_hi x W_lo
 //    into columns [BN, 2 BN) of one register accumulator, all as N = BN wgmma; the epilogue adds the halves.
-//  * Pixels on N (kPxN: Cout = 64, 64-channel chunks): a Cout = 64 layer would issue m64n64k16 with both operands read
-//    from shared memory, 4 KiB of operand reads per 64x64x16 MACs.  This form computes D^T = W_tap x A^T instead: the
-//    weight tap [64 x 64] is the A operand, the activation box the B operand, and each consumer warpgroup owns 128
-//    pixels (16 tile rows of 8) of a 32x8 tile, so every product is one m64n128k16 (3 KiB per 64x64x16 MACs, the
-//    ratio of the BN = 128 layers) and each weight tap serves 256 pixels.  The three products of the three-pass form
-//    share one accumulator.  The transposed accumulator holds couts on its rows: the epilogue stages each plane
-//    through shared memory with stmatrix.trans and stores whole 128-byte pixels; the fused 2x2 pool finds its
-//    partners in the thread's own registers (column e ^ 1, row j + 1).
+//  * Pixels on N (kPxN: BN = 64 or 128, 64-channel chunks): a Cout = 64 layer would issue m64n64k16 with both operands
+//    read from shared memory, 4 KiB of operand reads per 64x64x16 MACs.  This form computes D^T = W_tap x A^T instead:
+//    each 64-row half of the weight tap [BN x 64] is an M = 64 A operand, the activation box the B operand, and each
+//    consumer warpgroup owns 128 pixels (16 tile rows of 8) of a 32x8 tile, so every product is one m64n128k16 per
+//    64-cout half (3 KiB per 64x64x16 MACs; BN = 128 pixels on M reads 6 KiB per 64x128x16) and each weight tap serves
+//    256 pixels instead of 128, half the L2 -> SMEM weight traffic per MAC of the wide layers.  Cout = 256 / 512 run as
+//    2 / 4 N tiles of 128.  The three products of the three-pass form share one accumulator per half (the engine runs
+//    only single-pass layers at BN = 128: no register room to keep the cross products apart).  The transposed
+//    accumulator holds couts on its rows: the epilogue stages each plane and 64-cout half through shared memory with
+//    stmatrix.trans and stores whole 128-byte pixel rows; the fused 2x2 pool finds its partners in the thread's own
+//    registers (column e ^ 1, row j + 1).
 //
 // Roles: warp 8 (warpgroup 2, registers handed to the consumers) = TMA producer (+ L2 prefetch of the next tile's boxes; warp-uniform, one elected lane issues),
 // warps 0-7 = two consumer warpgroups, each owning 64 (kPxN: 128) pixels of the tile: wgmma into register
@@ -75,10 +78,11 @@ __host__ __device__ inline int w_tap_bytes(int bn, int kc, int planes = 2) { ret
 // 10-of-64 "side" source, the 3-of-32 image block); the all-zero k-steps are skipped, and with kPxN the source's weights
 // come packed one K block per dx column (film_pack.h), so each block serves three taps; kHalo = wide halo boxes; kOne =
 // single-pass product A_hi x W_hi (hi planes only); kRes = resident weights issued as straight-line code (a whole
-// activation stage is one wgmma group); kPxN = pixels on N (BN = 64, KC = 64, 32x8 tiles, store / pool epilogue only).
+// activation stage is one wgmma group); kPxN = pixels on N (BN = 64 or 128, KC = 64, 32x8 tiles, store / pool epilogue
+// only).
 template <int BN, int KC, bool kPartial, bool kHalo, bool kOne, bool kRes, bool kPxN = false>
 __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* __restrict__ prob) {
-  static_assert(!kPxN || (BN == 64 && KC == 64), "pixels on N: Cout = 64 (one M = 64 weight tile), 64-channel chunks");
+  static_assert(!kPxN || ((BN == 64 || BN == 128) && KC == 64), "pixels on N: one or two M = 64 weight tiles, 64-channel chunks");
   extern __shared__ uint8_t smem_raw[];
   constexpr bool one = kOne;
   const int planes = one ? 1 : 2;
@@ -92,7 +96,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
   const int kAStage = planes * kAPlane;
   const int kRowStep = kTileW * KC * 2;  // one tile row of pixels = tile_w/8 swizzle atoms
   constexpr bool kFused = BN <= 128 && !kPxN;
-  constexpr int kAccRegs = kPxN ? 64 : (kFused ? 2 * BN : BN) / 2;   // kPxN: m64n128 f32
+  constexpr int kMh = kPxN ? BN / 64 : 1;                            // kPxN: M = 64 halves of the weight tile
+  constexpr int kAccRegs = kPxN ? 64 * kMh : (kFused ? 2 * BN : BN) / 2;   // kPxN: one m64n128 f32 per half
   constexpr int kWgPx = kPxN ? 128 : 64;                              // pixels per consumer warpgroup
 
   // ---- problem fields -> registers, once (the asm "memory" clobbers would otherwise force a
@@ -320,6 +325,19 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
     const uint32_t sbo = kHalo ? kHaloW * kPx : 8 * kPx;
     RingPos ra, rw;   // activation / weight ring positions
     float acc[kAccRegs];
+    // pixels on N: half h of the weight tap (rows 64 h .. 64 h + 63, one 8 KiB run of 1 KiB swizzle atoms) into
+    // accumulator registers [64 h, 64 h + 64)
+    auto pxn_mma = [&](uint64_t w_hi, uint64_t w_lo, uint64_t a_hi, uint64_t a_lo, uint32_t accf) {
+#pragma unroll
+      for (int h = 0; h < kMh; ++h) {
+        const uint64_t wh = (uint64_t)(h * (64 * KC * 2) >> 4);
+        wgmma<128>(acc + 64 * h, w_hi + wh, a_hi, accf);
+        if constexpr (!kOne) {
+          wgmma<128>(acc + 64 * h, w_lo + wh, a_hi, 1u);
+          wgmma<128>(acc + 64 * h, w_hi + wh, a_lo, 1u);
+        }
+      }
+    };
     for (int tile = w_first; tile < nwork; tile += w_step) {
       int kb = 0;
       int rel_a = -1, rel_w = -1;   // stages read by the previous wgmma group, released once it retired
@@ -362,12 +380,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
             for (int k = 0; k < kSteps; ++k) {
               const uint64_t adv = (uint64_t)(k * 32 >> 4);
               const uint32_t accf = (t == 0 && k == 0) ? first : 1u;
-              if constexpr (kPxN) {   // D^T += W x A^T: the weight tap is the M = 64 operand
-                wgmma<128>(acc, w_hi + adv, a_hi + adv, accf);
-                if constexpr (!kOne) {
-                  wgmma<128>(acc, w_lo + adv, a_hi + adv, 1u);
-                  wgmma<128>(acc, w_hi + adv, a_lo + adv, 1u);
-                }
+              if constexpr (kPxN) {   // D^T += W x A^T: each 64-row half of the weight tap is an M = 64 operand
+                pxn_mma(w_hi + adv, w_lo + adv, a_hi + adv, a_lo + adv, accf);
               } else if constexpr (kOne) {
                 wgmma<BN>(acc, a_hi + adv, w_hi + adv, accf);
               } else if constexpr (kFused) {
@@ -409,11 +423,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
                 const uint64_t adv = (uint64_t)(k * 32 >> 4);
                 const uint32_t accf = (u == 0 && k == 0) ? first : 1u;
                 if constexpr (kPxN) {
-                  wgmma<128>(acc, w_hi + adv, a_hi + adv, accf);
-                  if constexpr (!kOne) {
-                    wgmma<128>(acc, w_lo + adv, a_hi + adv, 1u);
-                    wgmma<128>(acc, w_hi + adv, a_lo + adv, 1u);
-                  }
+                  pxn_mma(w_hi + adv, w_lo + adv, a_hi + adv, a_lo + adv, accf);
                 } else if constexpr (kOne) {
                   wgmma<BN>(acc, a_hi + adv, w_hi + adv, accf);
                 } else if constexpr (kFused) {
@@ -458,13 +468,17 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
       const int n0 = nti * BN;
       const bool live = sp < nsp;   // false: the empty partner of an odd tile count stores nothing
       if constexpr (kPxN) {
-        // Transposed accumulator: register 4j + 2h + e holds cout c0 + 8h and pixel (tile row 16 wg + j, column 2q + e)
+        // Transposed accumulator: register 64 m + 4j + 2h + e holds cout n0 + 64 m + c0 + 8h and pixel (tile row
+        // 16 wg + j, column 2q + e)
         const int c0 = 16 * (warp & 3) + (lane >> 2);
-        const float bias0 = bias_smem[c0], bias1 = bias_smem[c0 + 8];
 #pragma unroll
-        for (int i = 0; i < kAccRegs; ++i) {
-          const float f = acc[i] + ((i & 2) ? bias1 : bias0);
-          acc[i] = act ? leaky(f) : f;
+        for (int m = 0; m < kMh; ++m) {
+          const float bias0 = bias_smem[n0 + 64 * m + c0], bias1 = bias_smem[n0 + 64 * m + c0 + 8];
+#pragma unroll
+          for (int i = 64 * m; i < 64 * m + 64; ++i) {
+            const float f = acc[i] + ((i & 2) ? bias1 : bias0);
+            acc[i] = act ? leaky(f) : f;
+          }
         }
         const int y_wg = ty * kTileH + 16 * wg, x_t = tx * kTileW;
         if (do_pool) {
@@ -478,60 +492,65 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
             const bool ok = live && (py >> 1) < (out_H >> 1) && (px >> 1) < (out_W >> 1) && !(lane & 4);
             const int64_t ppix = ((int64_t)b * (out_H >> 1) + (py >> 1)) * (out_W >> 1) + (px >> 1);
 #pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              const int i = 4 * j + 2 * h;
-              const float v = ((acc[i] + acc[i + 1]) + (acc[i + 4] + acc[i + 5])) * 0.25f;
-              const float vn = __shfl_xor_sync(0xffffffffu, v, 4);
-              if (ok) {
-                uint32_t hi, lo;
-                split_pack2(v, vn, hi, lo);
-                *reinterpret_cast<uint32_t*>(pool_hi + ppix * pool_C + c0 + 8 * h) = hi;
-                *reinterpret_cast<uint32_t*>(pool_lo + ppix * pool_C + c0 + 8 * h) = lo;
+            for (int m = 0; m < kMh; ++m)
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int i = 64 * m + 4 * j + 2 * h;
+                const float v = ((acc[i] + acc[i + 1]) + (acc[i + 4] + acc[i + 5])) * 0.25f;
+                const float vn = __shfl_xor_sync(0xffffffffu, v, 4);
+                if (ok) {
+                  uint32_t hi, lo;
+                  split_pack2(v, vn, hi, lo);
+                  const int64_t pc = ppix * pool_C + n0 + 64 * m + c0 + 8 * h;
+                  *reinterpret_cast<uint32_t*>(pool_hi + pc) = hi;
+                  *reinterpret_cast<uint32_t*>(pool_lo + pc) = lo;
+                }
               }
-            }
           }
         }
-        // Split store: each plane goes through shared memory 64 pixels at a time.  stmatrix.trans writes 8 couts of one
-        // pixel as one 16-byte row (chunk cout / 8 of the pixel's 128 bytes, XOR-swizzled by pixel % 8: conflict-free);
-        // eight consecutive threads then store one pixel's 128 bytes
+        // Split store: each plane and 64-cout half goes through shared memory 64 pixels at a time.  stmatrix.trans
+        // writes 8 couts of one pixel as one 16-byte row (chunk cout / 8 of the pixel's 128 bytes, XOR-swizzled by
+        // pixel % 8: conflict-free); eight consecutive threads then store one pixel's 128 bytes of the half
         uint8_t* const stg = reinterpret_cast<uint8_t*>(src_tab) + 64 + wg * kPxnStageWg;
         const uint32_t stg_u = smem_u32(stg);
         const int t128 = threadIdx.x & 127;
         auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); };
         for (int pl = 0; pl < (lo_skip ? 1 : 2); ++pl) {
-          sp_t* const dst = pl ? out_lo : out_hi;
+          sp_t* const dst = (pl ? out_lo : out_hi) + out_c_off + n0;
 #pragma unroll
-          for (int half = 0; half < 2; ++half) {
-            wg_sync();   // the previous round's reads are done
+          for (int m = 0; m < kMh; ++m)
 #pragma unroll
-            for (int jj = 0; jj < 8; jj += 2) {
-              uint32_t r[4];   // matrices (j, h) = (jj, 0), (jj, 1), (jj + 1, 0), (jj + 1, 1)
+            for (int half = 0; half < 2; ++half) {
+              wg_sync();   // the previous round's reads are done
 #pragma unroll
-              for (int m = 0; m < 4; ++m) {
-                const int i = 4 * (8 * half + jj + (m >> 1)) + 2 * (m & 1);
-                if (pl) {
-                  uint32_t hi;
-                  split_pack2(acc[i], acc[i + 1], hi, r[m]);
-                } else {
-                  r[m] = pack2_hi(acc[i], acc[i + 1]);
+              for (int jj = 0; jj < 8; jj += 2) {
+                uint32_t r[4];   // matrices (j, h) = (jj, 0), (jj, 1), (jj + 1, 0), (jj + 1, 1)
+#pragma unroll
+                for (int mm = 0; mm < 4; ++mm) {
+                  const int i = 64 * m + 4 * (8 * half + jj + (mm >> 1)) + 2 * (mm & 1);
+                  if (pl) {
+                    uint32_t hi;
+                    split_pack2(acc[i], acc[i + 1], hi, r[mm]);
+                  } else {
+                    r[mm] = pack2_hi(acc[i], acc[i + 1]);
+                  }
+                }
+                // this lane addresses row (lane & 7) of matrix lane >> 3: pixel 8 (jj + lane / 16) + lane % 8 of the half
+                const int p = 8 * (jj + (lane >> 4)) + (lane & 7), ch = 2 * (warp & 3) + ((lane >> 3) & 1);
+                stmatrix_x4_trans(stg_u + p * 128 + ((ch ^ (p & 7)) << 4), r[0], r[1], r[2], r[3]);
+              }
+              wg_sync();
+#pragma unroll
+              for (int k = 0; k < 4; ++k) {
+                const int idx = 128 * k + t128, p = idx >> 3, ch = idx & 7;
+                const int py = y_wg + 8 * half + (p >> 3), px = x_t + (p & 7);
+                if (live && py < H && px < W) {
+                  const uint4 v = *reinterpret_cast<const uint4*>(stg + p * 128 + ((ch ^ (p & 7)) << 4));
+                  const int64_t opix = ((int64_t)b * out_H + py) * out_W + px;
+                  *reinterpret_cast<uint4*>(dst + opix * out_C + 64 * m + 8 * ch) = v;
                 }
               }
-              // this lane addresses row (lane & 7) of matrix lane >> 3: pixel 8 (jj + lane / 16) + lane % 8 of the half
-              const int p = 8 * (jj + (lane >> 4)) + (lane & 7), ch = 2 * (warp & 3) + ((lane >> 3) & 1);
-              stmatrix_x4_trans(stg_u + p * 128 + ((ch ^ (p & 7)) << 4), r[0], r[1], r[2], r[3]);
             }
-            wg_sync();
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const int idx = 128 * k + t128, p = idx >> 3, ch = idx & 7;
-              const int py = y_wg + 8 * half + (p >> 3), px = x_t + (p & 7);
-              if (live && py < H && px < W) {
-                const uint4 v = *reinterpret_cast<const uint4*>(stg + p * 128 + ((ch ^ (p & 7)) << 4));
-                const int64_t opix = ((int64_t)b * out_H + py) * out_W + px;
-                *reinterpret_cast<uint4*>(dst + opix * out_C + out_c_off + 8 * ch) = v;
-              }
-            }
-          }
         }
         continue;
       }
@@ -831,6 +850,8 @@ cudaError_t conv3x3_tc_configure() {
 #undef FILM_CFG
   e = Variants<64, 64, true>::configure();
   if (e != cudaSuccess) return e;
+  e = Variants<128, 64, true>::configure();
+  if (e != cudaSuccess) return e;
   return cudaSuccess;
 }
 
@@ -843,7 +864,7 @@ cudaError_t launch_conv3x3_tc(const ConvProblem* d_prob, const ConvProblem& h, c
   }
   switch (bn) {
     case 256: return Variants<256, 64>::launch(d_prob, h, st);
-    case 128: return Variants<128, 64>::launch(d_prob, h, st);
+    case 128: return h.pxn ? Variants<128, 64, true>::launch(d_prob, h, st) : Variants<128, 64>::launch(d_prob, h, st);
     case 64: return h.pxn ? Variants<64, 64, true>::launch(d_prob, h, st) : Variants<64, 64>::launch(d_prob, h, st);
     default: return Variants<32, 64>::launch(d_prob, h, st);
   }

@@ -88,8 +88,9 @@ struct Options {
                          // step 60.5 ms with them against 53.4 ms without (H100 SXM, 400 W; the paired layers run slower)
   int conv3x3_halo = 3;  // wide halo boxes (one 10-px box per chunk serves nine taps): 0 off, 1 the CTA-pair layers, 2 every
                          // 64-channel-chunk layer of the persistent kernel, 3 also its 32-channel-chunk layers
-  int conv3x3_pxn = 1;   // pixels on N for the Cout = 64 persistent 3x3 layers: 0 off, 1 where 32x8 tiles give two waves
-                         // over the SMs, k-step-skipping layers where they take half the waves of 16x8 tiles (default),
+  int conv3x3_pxn = 1;   // pixels on N for the Cout = 64 and single-pass Cout = 128 / 256 / 512 persistent 3x3 layers:
+                         // 0 off, 1 where 32x8 tiles give two waves over the SMs and the layer class measured faster
+                         // (add_conv), k-step-skipping layers where they take half the waves of 16x8 tiles (default),
                          // 2 every eligible layer
   int onepass_mask = (int)kDefaultOnepassMask;  // precision plan: stages on the single-pass product (see `enum Stage`)
   int fe_conv0_tc = 0;   // cfeat_conv_0: 0 = fp32 FMA kernel straight from the fp32 image (exact fp32, no widened image
@@ -715,9 +716,24 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   bool skips_ksteps = false;
   for (size_t s = 0; s < pc.src_chunks.size(); ++s)
     if (pc.src_chunks[s] > 0 && pc.src_ksteps[s] != kc / 16) skips_ksteps = true;
-  const bool pxn_pays = skips_ksteps ? 2 * waves(pxn_tiles) <= waves(tiles16) : pxn_tiles >= 2L * P.num_sms;
-  cp.pxn = (v2 && o.conv3x3_pxn && pc.cout == 64 && kc == kChunk && epi_mode == 0 && out && out_c_off % 8 == 0 &&
-            out->C % 8 == 0 && (!pool_out || pool_out->C % 8 == 0) && (o.conv3x3_pxn >= 2 || pxn_pays)) ? 1 : 0;
+  // Cout = 128 / 256 / 512 run as 1 / 2 / 4 N tiles of 128 couts, and count those towards the two waves.  Only
+  // single-pass ones move: with two M = 64 halves there is no register room to keep the hi x lo cross products apart,
+  // and the all-three-pass plan at 256x320 then moved 2.2e-5 from the per-tap generic kernel, over the 2e-5 its
+  // three-pass Cout = 64 layers keep.  Their sources must issue every k-step: the fusion_conv1 side source keeps its
+  // per-tap weight blocks on the 16x8 form.  By default only the classes that measured faster at 1088x1920 move (H100
+  // SXM, 700 W, ms on 16x8 tiles -> pixels on N):
+  //  * Cout = 128: fe_conv3@L1 1.200 -> 0.754, fe_conv2@L1 0.482 -> 0.328, flow_conv0@L2 0.958 -> 0.857.
+  //  * Cout = 256 with K <= 9216: fe_conv5@L2 0.785 -> 0.600, fusion_conv2@L2 0.364 -> 0.300.  flow_conv0@L3
+  //    (K = 17280) already issues ~700 TFLOP/s with BN = 256 and loses: 0.828 -> 0.941.
+  //  * Cout = 512 measured no gain: fe_conv7@L3 0.559 -> 0.562, fusion_conv2@L3 0.260 -> 0.276.
+  const bool wide = (pc.cout == 128 || pc.cout == 256 || pc.cout == 512) && cp.passes == 1 && !skips_ksteps;
+  const bool wide_pays = pc.cout == 128 || (pc.cout == 256 && pc.ktot <= 9 * 1024);
+  const long pxn_items = pxn_tiles * (wide ? pc.cout / 128 : 1);
+  const bool pxn_pays = skips_ksteps ? 2 * waves(pxn_tiles) <= waves(tiles16)
+                                     : pxn_items >= 2L * P.num_sms && (pc.cout == 64 || wide_pays);
+  cp.pxn = (v2 && o.conv3x3_pxn && (pc.cout == 64 || wide) && kc == kChunk && epi_mode == 0 && out &&
+            out_c_off % 8 == 0 && out->C % 8 == 0 && (!pool_out || pool_out->C % 8 == 0) &&
+            (o.conv3x3_pxn >= 2 || pxn_pays)) ? 1 : 0;
   // the pixels-on-N kernel reads a one-k-step source's weights packed per dx column, every other kernel per tap
   const int ktot = cp.pxn ? pc.pxn_ktot : pc.ktot;
   const sp_t* w_hi = cp.pxn ? pc.pxn_hi : pc.w_hi;
@@ -767,6 +783,7 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   cp.cout = pc.cout;
   cp.act = act;
   int bn = conv_tc_block_n(pc.cout);
+  if (cp.pxn && bn > 128) bn = 128;   // pixels on N: at most two M = 64 halves per weight tile
   if (out && !pool_out) {
     // tiny pyramid levels: a 17x30 level has 8 tiles but K = 17280 -- split N into smaller tiles so the
     // K-serial work spreads over more SMs (and BN <= 128 tiles use the 2-instruction product)

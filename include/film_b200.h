@@ -218,10 +218,13 @@ FILM_API int film_profile(film_handle* h, film_profile_t* out);
  *   "conv3x3_halo": wide halo boxes of the persistent kernel -- one (64 ch, 10 px, 18 rows) TMA box per chunk serves all
  *                   nine taps (wgmma descriptors at pixel offsets): 3 = 64- and 32-channel chunks (default),
  *                   2 = 64-channel chunks only, 1 = CTA-pair layers only, 0 = three dx-shifted 8-px boxes
- *   "conv3x3_pxn" : persistent 3x3 layers with Cout = 64, 64-channel chunks and a plain or pooled store put the pixels
- *                   on the wgmma N dimension (m64n128k16, weight tap as the M operand, 32x8 tiles): 1 = where 32x8 tiles
- *                   still give two waves over the SMs, and for a layer with a source that skips k-steps (fusion conv_1)
- *                   where they take at most half the waves of 16x8 tiles (default), 2 = every such layer, 0 = off
+ *   "conv3x3_pxn" : persistent 3x3 layers with Cout = 64 (or single-pass with Cout = 128, 256 or 512), 64-channel chunks
+ *                   and a plain or pooled store put the pixels on the wgmma N dimension (m64n128k16 per 64-cout half of
+ *                   a 128-cout N tile, weight tap as the M operand, 32x8 tiles): 1 = where 32x8 tiles times N tiles
+ *                   still give two waves over the SMs and the layer class measured faster (Cout = 64 and 128; Cout =
+ *                   256 with K <= 9216), and for a Cout = 64 layer with a source that skips k-steps (fusion conv_1)
+ *                   where 32x8 tiles take at most half the waves of 16x8 tiles (default), 2 = every such layer, 0 = off.
+ *                   Wider layers whose source skips k-steps keep the 16x8 form
  *   "fe_conv0_tc" : cfeat_conv_0 (3 -> 64, K = 27): 0 = register-tiled fp32 FMA kernel reading the fp32 image directly
  *                   (default: exact fp32 arithmetic, no widened image tensor), 1 = tensor-core kernel over a 32-channel-
  *                   padded split image
