@@ -25,10 +25,18 @@
 //    accumulator holds couts on its rows: the epilogue stages each plane and 64-cout half through shared memory with
 //    stmatrix.trans and stores whole 128-byte pixel rows; the fused 2x2 pool finds its partners in the thread's own
 //    registers (column e ^ 1, row j + 1).
+//  * Folded pixels on N (kPxN with BN = 32: the single-pass Cout = 32 convs of the level-0 flow predictor, KC = 64 or
+//    32): 32 couts fill only half of M = 64, and m64n32k16 pixels-on-M products read 3 KiB of operands per 32K MACs.
+//    Instead one [64 x KC] weight block holds two dy taps of a dx column (rows 0-31 tap dy, rows 32-63 tap dy + 1;
+//    film_pack.h), and each warpgroup issues one m64n136k16 over 17 tile rows of the box at tap dy's offset: rows 0-31
+//    of the accumulator hold its 16 output rows, rows 32-63 partial sums of the output one tile row up.  Per dx column
+//    the pairs are (-1, 0) and (zero weights, +1), six products per chunk instead of nine taps.  The epilogue stages the
+//    fp32 sums through shared memory, adds the lower half one pixel row up, and finishes one pixel per thread: the
+//    split store, or the fused flow head (conv_3, conv_4 and the residual add) with its weights read as broadcasts.
 //
 // Roles: warp 8 (warpgroup 2, registers handed to the consumers) = TMA producer (+ L2 prefetch of the next tile's boxes; warp-uniform, one elected lane issues),
 // warps 0-7 = two consumer warpgroups, each owning 64 (kPxN: 128) pixels of the tile: wgmma into register
-// accumulators, then the epilogue straight from the registers.
+// accumulators, then the epilogue from the registers (folded Cout = 32: through shared memory).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -68,9 +76,19 @@ constexpr int kHeadBytes = kHeadW3 + kHeadMisc;
 // kPxN store epilogue, after the src table: per consumer warpgroup one plane of 64 pixels x 64 channels
 constexpr int kPxnStageWg = 64 * 64 * 2;
 constexpr int kPxnStageBytes = 2 * kPxnStageWg;
+// folded Cout = 32 pixels-on-N epilogue, after the src table (and the flow head's scratch): per consumer warpgroup the
+// fp32 sums of 32 couts x 128 pixels, rows 136 floats apart (conflict-free float2 stores from the fragments and
+// conflict-free per-pixel reads)
+constexpr int kFoldLd = 136;
+constexpr int kFoldStageWg = 32 * kFoldLd * 4;
 // shared memory of the epilogue scratch after the src table
-inline int epi_scratch_bytes(int epi_mode, int pxn) { return epi_mode == 3 ? kHeadBytes : pxn ? kPxnStageBytes : 0; }
+inline int epi_scratch_bytes(int epi_mode, int pxn, int bn) {
+  if (pxn && bn == 32) return (epi_mode == 3 ? kHeadBytes : 0) + 2 * kFoldStageWg;
+  return epi_mode == 3 ? kHeadBytes : pxn ? kPxnStageBytes : 0;
+}
 
+// weight rows of one K block: BN, except the folded Cout = 32 pixels-on-N form, whose block holds two dy taps' 32 rows
+__host__ __device__ constexpr int w_rows(int bn, int pxn) { return pxn && bn == 32 ? 64 : bn; }
 __host__ __device__ inline int w_tap_bytes(int bn, int kc, int planes = 2) { return bn * kc * 2 * planes; }  // [BN x KC] hi (+ lo)
 
 // Variants are template parameters chosen on the host (launch_conv3x3_tc): kPartial = the activation stages
@@ -79,14 +97,20 @@ __host__ __device__ inline int w_tap_bytes(int bn, int kc, int planes = 2) { ret
 // come packed one K block per dx column (film_pack.h), so each block serves three taps; kHalo = wide halo boxes; kOne =
 // single-pass product A_hi x W_hi (hi planes only); kRes = resident weights issued as straight-line code (a whole
 // activation stage is one wgmma group); kPxN = pixels on N (BN = 64 or 128, KC = 64, 32x8 tiles, store / pool epilogue
-// only).
+// only; BN = 32: the folded form, KC = 64 or 32, single-pass, store or flow-head epilogue).
 template <int BN, int KC, bool kPartial, bool kHalo, bool kOne, bool kRes, bool kPxN = false>
 __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* __restrict__ prob) {
-  static_assert(!kPxN || ((BN == 64 || BN == 128) && KC == 64), "pixels on N: one or two M = 64 weight tiles, 64-channel chunks");
+  static_assert(!kPxN || ((BN == 64 || BN == 128) && KC == 64) || (BN == 32 && kOne && !kPartial),
+                "pixels on N: one or two M = 64 weight tiles of 64-channel chunks, or the folded single-pass Cout = 32 form");
   extern __shared__ uint8_t smem_raw[];
   constexpr bool one = kOne;
   const int planes = one ? 1 : 2;
-  constexpr int kWPlane = BN * KC * 2;  // one weight plane of one tap
+  // folded Cout = 32 pixels on N: each K block [64 x KC] holds two dy taps of one dx column, rows 0-31 tap dy and rows
+  // 32-63 tap dy + 1, and every product is one m64n136k16 over 17 tile rows of the box at the offset of tap dy.  Rows
+  // 32-63 then hold partial sums of the output one tile row up.  The pairs are (-1, 0) and (zero weights, +1): the
+  // third tap read at the dy = 0 offset keeps the 17 rows inside the box, where zero weights never meet unloaded bytes
+  constexpr bool kFold = kPxN && BN == 32;
+  constexpr int kWPlane = w_rows(BN, kPxN) * KC * 2;  // one weight plane of one K block
   const int kWTap = kWPlane * planes;
   const int kTileH = prob->tile_h, kTileW = prob->tile_w;
   constexpr int kHaloTileH = kPxN ? 32 : 16;   // the only tile height of a wide-halo box
@@ -96,8 +120,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
   const int kAStage = planes * kAPlane;
   const int kRowStep = kTileW * KC * 2;  // one tile row of pixels = tile_w/8 swizzle atoms
   constexpr bool kFused = BN <= 128 && !kPxN;
-  constexpr int kMh = kPxN ? BN / 64 : 1;                            // kPxN: M = 64 halves of the weight tile
-  constexpr int kAccRegs = kPxN ? 64 * kMh : (kFused ? 2 * BN : BN) / 2;   // kPxN: one m64n128 f32 per half
+  constexpr int kMh = kPxN && !kFold ? BN / 64 : 1;                   // kPxN: M = 64 halves of the weight tile
+  constexpr int kPxnN = kFold ? 136 : 128;                            // kPxN: pixel columns of one product
+  constexpr int kAccRegs = kPxN ? kPxnN / 2 * kMh : (kFused ? 2 * BN : BN) / 2;   // kPxN: one m64nN f32 per half
   constexpr int kWgPx = kPxN ? 128 : 64;                              // pixels per consumer warpgroup
 
   // ---- problem fields -> registers, once (the asm "memory" clobbers would otherwise force a
@@ -110,6 +135,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
   const int n_nt = (cout + BN - 1) / BN;                       // N tiles (Cout = 512 -> 2)
   const int ntiles = prob->B * tiles_per_img * n_nt;            // work items (spatial, N), N fastest
   constexpr int kStageTaps = kHalo ? 9 : 3;                     // taps served by one activation stage
+  constexpr int kStageMmas = kFold ? 2 * kStageTaps / 3 : kStageTaps;   // products per stage: one per tap or dy pair
   // Pixels on N: the partial source's packed weight blocks each hold k-step 0 of the three dy taps of one dx column.
   // The 16x8 form keeps one block per tap: packing measured no faster there, and it made the BN = 128 and 256 partial
   // instantiations spill about three times as much
@@ -117,8 +143,9 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
   const int part_lo = prob->v2_part_lo, part_hi = prob->v2_part_hi;   // kPartial: 1-k-step stages
   int nab = 0;                                                  // activation stages: one halo box or three dx boxes per chunk
   for (int s = 0; s < nsrc; ++s) nab += prob->src[s].nchunk * (kHalo ? 1 : 3);
-  // K blocks, in consumption order (source, chunk, dx, dy): one per tap, one per three taps in a packed partial stage
-  const int nkb = nab * kStageTaps - (kPacked ? (part_hi - part_lo) * (kStageTaps - kStageTaps / 3) : 0);
+  // K blocks, in consumption order (source, chunk, dx, dy): one per tap, one per three taps in a packed partial stage,
+  // two per dx column when folded
+  const int nkb = nab * kStageMmas - (kPacked ? (part_hi - part_lo) * (kStageTaps - kStageTaps / 3) : 0);
 
   const FastDiv div_nt(n_nt, ntiles), div_img(tiles_per_img, ntiles), div_tx(tiles_x, ntiles);   // tile decode
   // CTA pair (prob->pair, launched as (2,1,1) clusters): the two CTAs of a cluster walk the same work list, each on its
@@ -242,7 +269,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
             if (!resident) {
               // weight blocks consumed against this activation stage: one per tap, one per dx column when packed
               const bool packed = kPacked && ab >= part_lo && ab < part_hi;
-              const int nblk = packed ? kStageTaps / 3 : kStageTaps;
+              const int nblk = packed ? kStageTaps / 3 : kStageMmas;
               for (int t = 0; t < nblk; ++t, ++kb) {
                 const int ws = rw.stage;
                 mbar_wait(tail + 8u * (3 * kMaxRing + ws), rw.phase ^ 1u);
@@ -325,16 +352,19 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
     const uint32_t sbo = kHalo ? kHaloW * kPx : 8 * kPx;
     RingPos ra, rw;   // activation / weight ring positions
     float acc[kAccRegs];
+    // tap (3 dx + dy, dx-major within the stage) whose box offset product m of an activation stage reads: the folded
+    // form's products read at the upper tap of their dy pair, (-1, 0) and (zero, +1) of each dx column
+    auto tap_of = [](int m) { return kFold ? (kHalo ? 3 * (m / 2) : 0) + m % 2 : m; };
     // pixels on N: half h of the weight tap (rows 64 h .. 64 h + 63, one 8 KiB run of 1 KiB swizzle atoms) into
     // accumulator registers [64 h, 64 h + 64)
     auto pxn_mma = [&](uint64_t w_hi, uint64_t w_lo, uint64_t a_hi, uint64_t a_lo, uint32_t accf) {
 #pragma unroll
       for (int h = 0; h < kMh; ++h) {
         const uint64_t wh = (uint64_t)(h * (64 * KC * 2) >> 4);
-        wgmma<128>(acc + 64 * h, w_hi + wh, a_hi, accf);
+        wgmma<kPxnN>(acc + 64 * h, w_hi + wh, a_hi, accf);
         if constexpr (!kOne) {
-          wgmma<128>(acc + 64 * h, w_lo + wh, a_hi, 1u);
-          wgmma<128>(acc + 64 * h, w_hi + wh, a_lo, 1u);
+          wgmma<kPxnN>(acc + 64 * h, w_lo + wh, a_hi, 1u);
+          wgmma<kPxnN>(acc + 64 * h, w_hi + wh, a_lo, 1u);
         }
       }
     };
@@ -356,7 +386,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
       // weight block, their k-steps back to back in it: 3 in a packed partial stage (k-step 0 of each dy tap), else 1
       auto stage = [&](auto ksteps_c, auto tpb_c) {
         constexpr int kSteps = decltype(ksteps_c)::value, kTpb = decltype(tpb_c)::value;
-        constexpr int kBlocks = kStageTaps / kTpb;   // weight blocks read against this stage
+        constexpr int kBlocks = kStageMmas / kTpb;   // weight blocks read against this stage
         const int st = ra.stage;
         mbar_wait(tail + 8u * st, ra.phase);
         const uint32_t sa = a_base + st * kAStage + a_row0;
@@ -371,15 +401,16 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
           const uint32_t first = (kb == 0) ? 0u : 1u;
           wgmma_fence();
 #pragma unroll
-          for (int t = 0; t < kStageTaps; ++t) {
+          for (int mi = 0; mi < kStageMmas; ++mi) {
+            const int t = tap_of(mi);
             const uint64_t a_hi = a0 + (kHalo ? (uint64_t)((((t % 3) * kHaloW + t / 3) * kPx) >> 4) : (uint64_t)t * row_delta);
             const uint64_t a_lo = a_hi + lo_delta;
-            const uint64_t w_hi = w0 + (uint64_t)(((t / kTpb) * kWTapC + (t % kTpb) * kSteps * 32) >> 4);
+            const uint64_t w_hi = w0 + (uint64_t)(((mi / kTpb) * kWTapC + (mi % kTpb) * kSteps * 32) >> 4);
             const uint64_t w_lo = w_hi + (uint64_t)(kWPlane >> 4);
 #pragma unroll
             for (int k = 0; k < kSteps; ++k) {
               const uint64_t adv = (uint64_t)(k * 32 >> 4);
-              const uint32_t accf = (t == 0 && k == 0) ? first : 1u;
+              const uint32_t accf = (mi == 0 && k == 0) ? first : 1u;
               if constexpr (kPxN) {   // D^T += W x A^T: each 64-row half of the weight tap is an M = 64 operand
                 pxn_mma(w_hi + adv, w_lo + adv, a_hi + adv, a_lo + adv, accf);
               } else if constexpr (kOne) {
@@ -412,7 +443,7 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
             wgmma_fence();
 #pragma unroll
             for (int u = 0; u < kTpb; ++u) {
-              const int t = blk * kTpb + u;
+              const int t = tap_of(blk * kTpb + u);
               const uint32_t off = kHalo ? (uint32_t)((t % 3) * kHaloW + t / 3) * kPx : (uint32_t)(t * kRowStep);
               const uint64_t a_hi = make_desc_sbo<KC>(sa + off, sbo);
               const uint64_t a_lo = make_desc_sbo<KC>(sa + lo_off + off, sbo);
@@ -467,7 +498,93 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
       div_tx.divmod(rem, ty, tx);
       const int n0 = nti * BN;
       const bool live = sp < nsp;   // false: the empty partner of an odd tile count stores nothing
-      if constexpr (kPxN) {
+      if constexpr (kFold) {
+        // Register 4j + 2h + e holds weight row 16 (warp & 3) + lane / 4 + 8h at box column j (tile row 16 wg + j for
+        // rows 0-31, 16 wg + j - 1 for rows 32-63, j = 0 .. 16) and pixel column 2q + e.  The upper warps store their
+        // rows' sums, the lower warps add theirs one tile row up, and then each thread finishes one pixel
+        float* const stg = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(src_tab) + 64 + (fhead ? kHeadBytes : 0) +
+                                                    wg * kFoldStageWg);
+        auto wg_sync = [&]() { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); };
+        const bool lower = (warp & 2) != 0;
+        const int r0 = 16 * (warp & 1) + (lane >> 2);
+        wg_sync();   // the previous tile's reads are done
+        if (!lower) {
+#pragma unroll
+          for (int j = 0; j < 16; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              *reinterpret_cast<float2*>(stg + (r0 + 8 * h) * kFoldLd + 8 * j + 2 * q) =
+                  make_float2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+        }
+        wg_sync();
+        if (lower) {
+#pragma unroll
+          for (int j = 1; j < 17; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              float2* d = reinterpret_cast<float2*>(stg + (r0 + 8 * h) * kFoldLd + 8 * (j - 1) + 2 * q);
+              const float2 v = *d;
+              *d = make_float2(v.x + acc[4 * j + 2 * h], v.y + acc[4 * j + 2 * h + 1]);
+            }
+        }
+        wg_sync();
+        const int p = threadIdx.x & 127;
+        const int py = ty * kTileH + 16 * wg + (p >> 3), px = tx * kTileW + (p & 7);
+        const int64_t opix = ((int64_t)b * out_H + py) * out_W + px;
+        float f[32];
+#pragma unroll
+        for (int c = 0; c < 32; ++c) {
+          const float x = stg[c * kFoldLd + p] + bias_smem[c];
+          f[c] = act ? leaky(x) : x;
+        }
+        if (!live || py >= H || px >= W) {
+        } else if (fhead) {
+          // conv_3 (32 -> 16, bias, LeakyReLU), conv_4 (16 -> 2) and the residual add of the flow head
+          float hp[16];
+#pragma unroll
+          for (int hh = 0; hh < 16; ++hh) hp[hh] = 0.f;
+#pragma unroll
+          for (int c = 0; c < 32; ++c) {
+            const float4* wr = reinterpret_cast<const float4*>(w3s + c * 16);
+#pragma unroll
+            for (int h4 = 0; h4 < 4; ++h4) {
+              const float4 wv = wr[h4];
+              hp[4 * h4] = fmaf(f[c], wv.x, hp[4 * h4]);
+              hp[4 * h4 + 1] = fmaf(f[c], wv.y, hp[4 * h4 + 1]);
+              hp[4 * h4 + 2] = fmaf(f[c], wv.z, hp[4 * h4 + 2]);
+              hp[4 * h4 + 3] = fmaf(f[c], wv.w, hp[4 * h4 + 3]);
+            }
+          }
+          float f0 = hmisc[3 * 16], f1 = hmisc[3 * 16 + 1];
+#pragma unroll
+          for (int hh = 0; hh < 16; ++hh) {
+            const float x = leaky(hp[hh] + hmisc[hh]);
+            f0 = fmaf(x, hmisc[16 + 2 * hh], f0);
+            f1 = fmaf(x, hmisc[16 + 2 * hh + 1], f1);
+          }
+          float2 res = make_float2(f0, f1), tot = res;
+          if (head_vup) {
+            const float2 u = reinterpret_cast<const float2*>(head_vup)[opix];
+            tot.x += u.x;
+            tot.y += u.y;
+          }
+          reinterpret_cast<float2*>(head_res)[opix] = res;
+          reinterpret_cast<float2*>(head_vout)[opix] = tot;
+        } else {
+          sp_t* const oh = out_hi + opix * out_C + out_c_off;
+          sp_t* const ol = out_lo + opix * out_C + out_c_off;
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            uint32_t hi[4], lo[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) split_pack2(f[8 * k + 2 * i], f[8 * k + 2 * i + 1], hi[i], lo[i]);
+            *reinterpret_cast<uint4*>(oh + 8 * k) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+            if (!lo_skip) *reinterpret_cast<uint4*>(ol + 8 * k) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+          }
+        }
+        continue;
+      }
+      if constexpr (kPxN && !kFold) {
         // Transposed accumulator: register 64 m + 4j + 2h + e holds cout n0 + 64 m + c0 + 8h and pixel (tile row
         // 16 wg + j, column 2q + e)
         const int c0 = 16 * (warp & 3) + (lane >> 2);
@@ -701,9 +818,10 @@ __global__ void __launch_bounds__(kThreads, 1) k_conv3x3_tc(const ConvProblem* _
 int smem_bytes_for(const ConvProblem& h, int bn) {
   const int nkb = h.ktot / h.kchunk;
   const int planes = h.passes == 1 ? 1 : 2;
-  const int w = h.v2_resident ? nkb * w_tap_bytes(bn, h.kchunk, planes) : h.v2_nw * w_tap_bytes(bn, h.kchunk, planes);
+  const int wtap = w_tap_bytes(w_rows(bn, h.pxn), h.kchunk, planes);
+  const int w = h.v2_resident ? nkb * wtap : h.v2_nw * wtap;
   return h.v2_na * a_stage_bytes_h(h.kchunk, h.tile_h, h.tile_w, h.halo, planes) + w + kFixedBytes +
-         epi_scratch_bytes(h.epi_mode, h.pxn);
+         epi_scratch_bytes(h.epi_mode, h.pxn, bn);
 }
 
 }  // namespace
@@ -717,9 +835,9 @@ namespace {
 // Returns false when the shape cannot get them within the shared-memory budget.
 bool ring_depths(int kc, int tile_h, int tile_w, int halo, int planes, int bn, int cout, int ktot, int epi_mode, int pxn,
                  int& resident, int& na, int& nw) {
-  const int wtap = w_tap_bytes(bn, kc, planes);
+  const int wtap = w_tap_bytes(w_rows(bn, pxn), kc, planes);
   const int w_all = (ktot / kc) * wtap;
-  const int kLimit = kSmemLimit - epi_scratch_bytes(epi_mode, pxn);   // flow-head / pixels-on-N store scratch
+  const int kLimit = kSmemLimit - epi_scratch_bytes(epi_mode, pxn, bn);   // flow-head / pixels-on-N store scratch
   const int kAStage = a_stage_bytes_h(kc, tile_h, tile_w, halo, planes);
   if (cout <= bn && w_all + 2 * kAStage + kFixedBytes <= kLimit) {
     resident = 1;
@@ -770,10 +888,10 @@ void conv3x3_tc_pick_tile(int H, int W, int B, int cout, int kc, int passes, int
 bool conv3x3_tc_plan(ConvProblem& h, int num_sms) {
   const int bn = h.bn;
   const int planes = h.passes == 1 ? 1 : 2;
-  const int wtap = w_tap_bytes(bn, h.kchunk, planes);
+  const int wtap = w_tap_bytes(w_rows(bn, h.pxn), h.kchunk, planes);
   const int w_all = (h.ktot / h.kchunk) * wtap;
   const bool can_resident = h.cout <= bn;
-  const int kLimit = kSmemLimit - epi_scratch_bytes(h.epi_mode, h.pxn);
+  const int kLimit = kSmemLimit - epi_scratch_bytes(h.epi_mode, h.pxn, bn);
   // wide halo (the engine allows it per chunk size): 16x8 (pixels on N: 32x8) tiles only; resident weights win when
   // both do not fit
   if (h.halo && (h.tile_h != (h.pxn ? 32 : 16) || h.tile_w != 8 ||
@@ -797,20 +915,31 @@ bool conv3x3_tc_plan(ConvProblem& h, int num_sms) {
   return ok;
 }
 
+using ConvKernel = void (*)(const ConvProblem*);
+// the folded Cout = 32 pixels-on-N form exists single-pass and without a k-step-skipping source only
+template <int BN, int KC, bool kPartial, bool kHalo, bool kOne, bool kRes, bool kPxN>
+constexpr ConvKernel kernel_of() {
+  if constexpr (kPxN && BN == 32 && (kPartial || !kOne))
+    return nullptr;
+  else
+    return k_conv3x3_tc<BN, KC, kPartial, kHalo, kOne, kRes, kPxN>;
+}
+
 template <int BN, int KC, bool kPxN = false>
 struct Variants {
   // every (kPartial, kHalo, kOne, kRes) instantiation of one (BN, KC, kPxN) kernel, indexed by the four bits
-  static constexpr void (*kFn[16])(const ConvProblem*) = {
-      k_conv3x3_tc<BN, KC, false, false, false, false, kPxN>, k_conv3x3_tc<BN, KC, false, false, false, true, kPxN>,
-      k_conv3x3_tc<BN, KC, false, false, true, false, kPxN>,  k_conv3x3_tc<BN, KC, false, false, true, true, kPxN>,
-      k_conv3x3_tc<BN, KC, false, true, false, false, kPxN>,  k_conv3x3_tc<BN, KC, false, true, false, true, kPxN>,
-      k_conv3x3_tc<BN, KC, false, true, true, false, kPxN>,   k_conv3x3_tc<BN, KC, false, true, true, true, kPxN>,
-      k_conv3x3_tc<BN, KC, true, false, false, false, kPxN>,  k_conv3x3_tc<BN, KC, true, false, false, true, kPxN>,
-      k_conv3x3_tc<BN, KC, true, false, true, false, kPxN>,   k_conv3x3_tc<BN, KC, true, false, true, true, kPxN>,
-      k_conv3x3_tc<BN, KC, true, true, false, false, kPxN>,   k_conv3x3_tc<BN, KC, true, true, false, true, kPxN>,
-      k_conv3x3_tc<BN, KC, true, true, true, false, kPxN>,    k_conv3x3_tc<BN, KC, true, true, true, true, kPxN>};
+  static constexpr ConvKernel kFn[16] = {
+      kernel_of<BN, KC, false, false, false, false, kPxN>(), kernel_of<BN, KC, false, false, false, true, kPxN>(),
+      kernel_of<BN, KC, false, false, true, false, kPxN>(),  kernel_of<BN, KC, false, false, true, true, kPxN>(),
+      kernel_of<BN, KC, false, true, false, false, kPxN>(),  kernel_of<BN, KC, false, true, false, true, kPxN>(),
+      kernel_of<BN, KC, false, true, true, false, kPxN>(),   kernel_of<BN, KC, false, true, true, true, kPxN>(),
+      kernel_of<BN, KC, true, false, false, false, kPxN>(),  kernel_of<BN, KC, true, false, false, true, kPxN>(),
+      kernel_of<BN, KC, true, false, true, false, kPxN>(),   kernel_of<BN, KC, true, false, true, true, kPxN>(),
+      kernel_of<BN, KC, true, true, false, false, kPxN>(),   kernel_of<BN, KC, true, true, false, true, kPxN>(),
+      kernel_of<BN, KC, true, true, true, false, kPxN>(),    kernel_of<BN, KC, true, true, true, true, kPxN>()};
   static cudaError_t configure() {
     for (auto fn : kFn) {
+      if (!fn) continue;
       const cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemLimit);
       if (e != cudaSuccess) return e;
     }
@@ -818,9 +947,12 @@ struct Variants {
   }
   static cudaError_t launch(const ConvProblem* d_prob, const ConvProblem& h, cudaStream_t st) {
     if (h.v2_na < 2 || (!h.v2_resident && h.v2_nw < 2)) return cudaErrorInvalidValue;   // see ring_depths
-    if (kPxN && (h.pair || h.tile_h != 32 || h.tile_w != 8 || h.epi_mode != 0)) return cudaErrorInvalidValue;
+    if (kPxN && (h.pair || h.tile_h != 32 || h.tile_w != 8 || h.epi_mode != (BN == 32 && h.epi_mode == 3 ? 3 : 0)))
+      return cudaErrorInvalidValue;
+    if (kPxN && BN == 32 && h.pool_hi) return cudaErrorInvalidValue;   // the folded form has no pool epilogue
     const bool partial = h.v2_part_hi > h.v2_part_lo;
     const int idx = (partial ? 8 : 0) | (h.halo ? 4 : 0) | (h.passes == 1 ? 2 : 0) | (h.v2_resident && h.straight ? 1 : 0);
+    if (!kFn[idx]) return cudaErrorInvalidValue;   // a form this kernel does not have
     if (!h.pair) {
       kFn[idx]<<<h.v2_grid, kThreads, smem_bytes_for(h, BN), st>>>(d_prob);
       return cudaGetLastError();
@@ -852,13 +984,17 @@ cudaError_t conv3x3_tc_configure() {
   if (e != cudaSuccess) return e;
   e = Variants<128, 64, true>::configure();
   if (e != cudaSuccess) return e;
+  e = Variants<32, 64, true>::configure();
+  if (e != cudaSuccess) return e;
+  e = Variants<32, 32, true>::configure();
+  if (e != cudaSuccess) return e;
   return cudaSuccess;
 }
 
 cudaError_t launch_conv3x3_tc(const ConvProblem* d_prob, const ConvProblem& h, cudaStream_t st) {
   const int bn = h.bn;
   if (h.kchunk == 32) {  // 32-channel K blocks: the 32 -> 32 flow convs and the 3(32) -> 64 first conv
-    if (bn == 32) return Variants<32, 32>::launch(d_prob, h, st);
+    if (bn == 32) return h.pxn ? Variants<32, 32, true>::launch(d_prob, h, st) : Variants<32, 32>::launch(d_prob, h, st);
     if (bn == 64) return Variants<64, 32>::launch(d_prob, h, st);
     return cudaErrorInvalidValue;
   }
@@ -866,7 +1002,7 @@ cudaError_t launch_conv3x3_tc(const ConvProblem* d_prob, const ConvProblem& h, c
     case 256: return Variants<256, 64>::launch(d_prob, h, st);
     case 128: return h.pxn ? Variants<128, 64, true>::launch(d_prob, h, st) : Variants<128, 64>::launch(d_prob, h, st);
     case 64: return h.pxn ? Variants<64, 64, true>::launch(d_prob, h, st) : Variants<64, 64>::launch(d_prob, h, st);
-    default: return Variants<32, 64>::launch(d_prob, h, st);
+    default: return h.pxn ? Variants<32, 64, true>::launch(d_prob, h, st) : Variants<32, 64>::launch(d_prob, h, st);
   }
 }
 

@@ -250,7 +250,7 @@ struct PackedConv {
   std::vector<int> src_chunks;  // K-block chunks per source
   std::vector<int> src_ksteps;  // 16-channel k-steps per chunk that hold at least one real channel
   // weights of the pixels-on-N 3x3 kernel: a one-k-step source with 64-channel chunks is packed one K block per dx
-  // column (film_pack.h); the same arrays as w_hi / w_lo when no source is packed
+  // column, a Cout = 32 conv as [64 x K] dy-pair blocks (film_pack.h); the same arrays as w_hi / w_lo otherwise
   sp_t* pxn_hi = nullptr;
   sp_t* pxn_lo = nullptr;
   int pxn_ktot = 0;
@@ -332,6 +332,10 @@ static PackedConv pack_conv(const HostTensor& kernel, const HostTensor& bias,
   if (std::count(packed.begin(), packed.end(), 1)) {
     pc.pxn_hi = upload(pack_dx_blocks(hi, cout, ktot, chunk, pc.src_chunks, packed, pc.pxn_ktot));
     pc.pxn_lo = upload(pack_dx_blocks(lo, cout, ktot, chunk, pc.src_chunks, packed, pc.pxn_ktot));
+  } else if (cout == 32 && taps.size() == 9) {   // the folded form: two dy taps per [64 x chunk] block
+    pc.pxn_hi = upload(pack_dy_pairs(hi, ktot, chunk));
+    pc.pxn_lo = upload(pack_dy_pairs(lo, ktot, chunk));
+    pc.pxn_ktot = ktot / 9 * 6;
   }
   FILM_CUDA(cudaMalloc(&pc.bias, cout * 4));
   allocs.push_back(pc.bias);
@@ -728,13 +732,20 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   //  * Cout = 512 measured no gain: fe_conv7@L3 0.559 -> 0.562, fusion_conv2@L3 0.260 -> 0.276.
   const bool wide = (pc.cout == 128 || pc.cout == 256 || pc.cout == 512) && cp.passes == 1 && !skips_ksteps;
   const bool wide_pays = pc.cout == 128 || (pc.cout == 256 && pc.ktot <= 9 * 1024);
+  // Cout = 32 (the level-0 flow predictor, 64- or 32-channel chunks): the folded form, two dy taps per M = 64 weight
+  // operand, with the store or the flow-head epilogue.  Single-pass layers only: three-pass ones would need the cross
+  // products in accumulators of their own.  At 1088x1920 (H100 SXM, 700 W), ms on 16x8 tiles -> folded:
+  // flow_conv0@L0 0.925 -> 0.689, flow_conv1@L0 0.528 -> 0.304, flow_conv2+head@L0 1.830 -> 0.446
+  const bool fold = pc.cout == 32 && cp.passes == 1 && !skips_ksteps && !pool_out && (epi_mode == 3 || (epi_mode == 0 && out));
   const long pxn_items = pxn_tiles * (wide ? pc.cout / 128 : 1);
   const bool pxn_pays = skips_ksteps ? 2 * waves(pxn_tiles) <= waves(tiles16)
-                                     : pxn_items >= 2L * P.num_sms && (pc.cout == 64 || wide_pays);
-  cp.pxn = (v2 && o.conv3x3_pxn && (pc.cout == 64 || wide) && kc == kChunk && epi_mode == 0 && out &&
-            out_c_off % 8 == 0 && out->C % 8 == 0 && (!pool_out || pool_out->C % 8 == 0) &&
+                                     : pxn_items >= 2L * P.num_sms && (pc.cout == 64 || wide_pays || fold);
+  const bool pxn_store = epi_mode == 0 && out && out_c_off % 8 == 0 && out->C % 8 == 0 && (!pool_out || pool_out->C % 8 == 0);
+  cp.pxn = (v2 && o.conv3x3_pxn && (((pc.cout == 64 || wide) && kc == kChunk && pxn_store) || (fold && (epi_mode == 3 || pxn_store))) &&
             (o.conv3x3_pxn >= 2 || pxn_pays)) ? 1 : 0;
-  // the pixels-on-N kernel reads a one-k-step source's weights packed per dx column, every other kernel per tap
+  // the pixels-on-N kernel reads a one-k-step source's weights packed per dx column and the folded form's weights packed
+  // per dy pair (film_pack.h), every other kernel per tap
+  const bool folded = cp.pxn && pc.cout == 32;
   const int ktot = cp.pxn ? pc.pxn_ktot : pc.ktot;
   const sp_t* w_hi = cp.pxn ? pc.pxn_hi : pc.w_hi;
   const sp_t* w_lo = cp.pxn ? pc.pxn_lo : pc.w_lo;
@@ -791,10 +802,11 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
     while (bn > 64 && 2 * items(bn) <= P.num_sms) bn /= 2;  // only while under half of the SMs have work
   }
   cp.bn = bn;
-  make_w_map(&cp.tm_w_hi, w_hi, pc.cout, ktot, bn, kc);
-  make_w_map(&cp.tm_w_lo, w_lo, pc.cout, ktot, bn, kc);
-  make_w_map(&cp.tm_w_hi_half, w_hi, pc.cout, ktot, bn / 2, kc);
-  make_w_map(&cp.tm_w_lo_half, w_lo, pc.cout, ktot, bn / 2, kc);
+  const int w_rows = folded ? 64 : pc.cout, w_box = folded ? 64 : bn;   // folded: [64 x K] blocks, two dy taps each
+  make_w_map(&cp.tm_w_hi, w_hi, w_rows, ktot, w_box, kc);
+  make_w_map(&cp.tm_w_lo, w_lo, w_rows, ktot, w_box, kc);
+  make_w_map(&cp.tm_w_hi_half, w_hi, w_rows, ktot, w_box / 2, kc);
+  make_w_map(&cp.tm_w_lo_half, w_lo, w_rows, ktot, w_box / 2, kc);
   if (out) {
     cp.out_hi = out->hi;
     cp.out_lo = out->lo;
@@ -864,8 +876,9 @@ static size_t add_conv(Plan& P, const std::string& tag, double ref_macs_per_px, 
   double k_issued = 0;  // skipped all-zero k-steps are not issued work
   for (size_t si = 0; si < pc.src_chunks.size(); ++si)
     k_issued += (double)pc.src_chunks[si] * pc.ntaps * (v2 ? pc.src_ksteps[si] * 16 : pc.kchunk);
+  // (the folded form issues six m64n136 products per warpgroup for nine taps of 32 couts x 128 pixels: 17/12 of them)
   P.mma_flops += (double)cp.passes * 2.0 * (double)cp.B * cp.tiles_y * cp.tiles_x * (cp.tile_h * cp.tile_w) * k_issued *
-                 (double)(((pc.cout + bn - 1) / bn) * bn);
+                 (double)(((pc.cout + bn - 1) / bn) * bn) * (folded ? 17.0 / 12.0 : 1.0);
   // algorithmic HBM bytes of this call site: every source plane it consumes read once, every destination plane written once
   double alg_bytes = 0;
   {

@@ -38,4 +38,24 @@ inline std::vector<uint16_t> pack_dx_blocks(const std::vector<uint16_t>& per_tap
   return out;
 }
 
+// Weight layout of the folded Cout = 32 pixels-on-N form of the persistent 3x3 kernel: one M = 64 operand holds two dy
+// taps of one dx column.  per_tap: [32][ktot] in the K order above.  Each (chunk, dx) gets two [64 x chunk] K blocks:
+// rows 0-31 tap dy = -1 and rows 32-63 tap dy = 0, then zero rows 0-31 and rows 32-63 tap dy = +1 (the kernel reads it
+// at the dy = 0 box offset, so its 17 tile rows stay inside the box).  Returns [64][ktot * 2 / 3].
+inline std::vector<uint16_t> pack_dy_pairs(const std::vector<uint16_t>& per_tap, int ktot, int chunk) {
+  const int ktot_out = ktot / 9 * 6;
+  std::vector<uint16_t> out((size_t)64 * ktot_out, 0);
+  for (int g = 0; g < ktot / (9 * chunk); ++g)
+    for (int dx = 0; dx < 3; ++dx)
+      for (int n = 0; n < 32; ++n)
+        for (int c = 0; c < chunk; ++c) {
+          const uint16_t* src = per_tap.data() + (size_t)n * ktot + (size_t)(g * 9 + 3 * dx) * chunk + c;
+          uint16_t* dst = out.data() + (size_t)(g * 6 + 2 * dx) * chunk + c;
+          dst[(size_t)n * ktot_out] = src[0];                                // dy = -1
+          dst[(size_t)(32 + n) * ktot_out] = src[chunk];                     // dy = 0
+          dst[(size_t)(32 + n) * ktot_out + chunk] = src[2 * chunk];         // dy = +1
+        }
+  return out;
+}
+
 }  // namespace film
